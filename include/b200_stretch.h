@@ -153,7 +153,8 @@ int b200s_profile_begin(b200s_engine *e);
 int b200s_profile_end(b200s_engine *e, float *ms, int *counts, int n);
 
 /* Device self-test: the branch-free division / square root of the phase chain against the IEEE
- * round-to-nearest intrinsics on `n` pseudo-random operand pairs; returns the mismatch counts. */
+ * round-to-nearest intrinsics, bit for bit, on `n` pseudo-random normal-range operand pairs plus `n` pairs from the
+ * edge classes (zero, subnormal and huge operands, infinite divisors); returns the mismatch counts. */
 int b200s_selftest_divsqrt(b200s_engine *e, long long n, long long seed, long long *div_mismatch, long long *sqrt_mismatch);
 
 /* ---- white-box state for teacher-forced parity tests (SURVEY.md section 8(c)) ----

@@ -29,9 +29,7 @@ namespace b200s {
 // recurrence is added last, a / b as a * rcp(b), phase * sqrt(energy / |phase|^2) as phase * (sqrt(energy) *
 // rsqrt(|phase|^2)) on the SFU approximations (1-2 ulp).  Results agree with the exact mode to float rounding per
 // operation; both are tested against the oracle to the north-star tolerance (tests/test_gpu_parity.py).
-#ifdef B200S_EMU
-__device__ __forceinline__ f2 neg2(f2 a) { return f2{-a.a, -a.b}; }
-#endif
+__device__ __forceinline__ f2 neg2(f2 a) { return f2_make(-f2_lo(a), -f2_hi(a)); } // folded into operand modifiers by ptxas
 // (the scalar fast helpers -- rcp_fast, rsqrt_fast, sqrt_fast, ffma, fmul_f, fmulc_f, make_output_fast -- live in kernels.cuh:
 //  the mono direct chain uses them too)
 // a * b and a * conj(b), fused

@@ -30,6 +30,37 @@ def batch(kind, S, C, n, sr):
     return np.stack([np.stack([gen(n, sr, s, c) for c in range(C)]) for s in range(S)])
 
 
+def edge(kind, S, C, n, sr):
+    """Inputs at the edges of the float range and of the spectrum, [S][C][n]:
+    harmonic_<scale>  the harmonic fixture times <scale> (32768: int16 sample values passed as float);
+    loud_and_tiny     channel 0 at int16 level, the others at 1e-20 (their energies fall below FLT_MIN);
+    loud_and_zero     channel 0 at int16 level, the others exactly zero;
+    dc / nyquist      full-scale constant / +-1 alternating every sample;
+    impulses          isolated unit impulses (one every 1999 samples, offset by the stream index);
+    impulse_train     a unit impulse every 7 samples: over 7 consecutive blocks some land on the first and on the last
+                      sample of the analysis window."""
+    x = batch("harmonic", S, C, n, sr)
+    if kind.startswith("harmonic_"):
+        return (x * np.float32(float(kind.split("_", 1)[1]))).astype(np.float32)
+    if kind in ("loud_and_tiny", "loud_and_zero"):
+        x[:, 0] *= np.float32(32768)
+        x[:, 1:] = x[:, 1:] * np.float32(1e-20) if kind == "loud_and_tiny" else 0.0
+        return x
+    x[:] = 0.0
+    if kind == "dc":
+        x[:] = 1.0
+    elif kind == "nyquist":
+        x[:] = np.where(np.arange(n) % 2 == 0, 1.0, -1.0).astype(np.float32)
+    elif kind == "impulses":
+        for s in range(S):
+            x[s, :, 500 + 37 * s::1999] = 1.0
+    elif kind == "impulse_train":
+        x[:, :, ::7] = 1.0
+    else:
+        raise ValueError(kind)
+    return x
+
+
 def chunks(n_in, ratio_out, chunk_out):
     """(in_start, in_len, out_len) per call so that every call keeps the exact in/out ratio."""
     n_out = int(round(n_in * ratio_out))

@@ -272,7 +272,9 @@ def test_device_pointer_api_matches_host_api(gpu):
 
 def test_fast_div_sqrt_are_correctly_rounded(gpu):
     """The branch-free division / square root of the chain kernel (kernels.cuh fdivq/fsqrtq) must equal
-    the IEEE round-to-nearest intrinsics bit for bit: 2^27 operand pairs, exponents 2^-60 .. 2^60."""
+    the IEEE round-to-nearest intrinsics bit for bit: 2^27 operand pairs, exponents 2^-60 .. 2^60, plus 2^27 pairs from the
+    edge classes (zero, subnormal, tiny and huge numerators, divisors up to FLT_MAX and +-inf, subnormal, zero and
+    infinite square-root arguments)."""
     e = gpu(1)
     bad_div, bad_sqrt = e.selftest_divsqrt(1 << 27, 12345)
     assert bad_div == 0 and bad_sqrt == 0, (bad_div, bad_sqrt)

@@ -661,6 +661,14 @@ def test_unsupported_features_fail_loudly(emu_libs):
         g.configure(3, 512, 128)
     with pytest.raises(StretchError, match="unknown key"):
         g.set_tuning(99, 0)
+    # 192 kHz presets: K = 12288 bands, beyond the shared-memory FFT (the largest size, 6144, is 96 kHz): refused with
+    # B200S_EUNSUPPORTED (-4) before anything is launched
+    g.presetDefault(1, 96000.0)
+    before = g.kernel_launches()
+    for preset in ("presetDefault", "presetCheaper"):
+        with pytest.raises(StretchError, match="error -4"):
+            getattr(g, preset)(1, 192000.0)
+    assert g.kernel_launches() == before and g.bands() == 6144
 
 
 def test_file_mode_caller_against_the_oracle(emu_libs, oracle_port, tmp_path):
