@@ -159,8 +159,8 @@ __global__ void __launch_bounds__(32) k_chain_direct4(Ctx x) {
 				const int fl = fillF + 4 * it;
 				const int q = kf + fillI - G * fl;
 				if (fl < nAct && (unsigned)q < (unsigned)K) {
-					cp_async16(&U.in[q & (CH3_RING - 1)][fl], rIn[it] + q);
-					cp_async16(&U.pvy[buf][fillI][fl], rPv[it] + q);
+					cp_async16_pf(&U.in[q & (CH3_RING - 1)][fl], rIn[it] + q);
+					cp_async16_pf(&U.pvy[buf][fillI][fl], rPv[it] + q);
 				}
 			}
 			if (lane < 2 * CHAIN_CH) { // lane 0's predecessor: planar state / previous group rows -> {c0, c1} slots
@@ -178,6 +178,9 @@ __global__ void __launch_bounds__(32) k_chain_direct4(Ctx x) {
 		};
 		fill(0, 0);
 		int cb = 0; // buffer of the chunk being computed
+		float4 carry[8]; // write-back: the previous chunk's finals of the next aligned piece (see the end of the chunk)
+#pragma unroll
+		for (int it = 0; it < 8; ++it) carry[it] = make_float4(0.f, 0.f, 0.f, 0.f);
 		for (int k0 = 0; k0 < steps; k0 += CHAIN_CH, cb ^= 1) {
 			cp_async_wait_all(); // this chunk's tiles (issued one chunk ago)
 			__syncwarp();
@@ -396,20 +399,38 @@ __global__ void __launch_bounds__(32) k_chain_direct4(Ctx x) {
 			else if (k0 >= interiorFrom && k0 + CHAIN_CH <= K) run_chunk(std::false_type{}, std::true_type{});
 			else run_chunk(std::false_type{}, std::false_type{});
 			__syncwarp();
-			// ---------------- write the chunk's finals back: planar Band::output rows, 32 B per row and quarter-warp;
-			//                  all tile reads first, then the stores (row addresses are arithmetic) ----------------
+			// ---------------- write the finals back: planar Band::output rows in whole 32-byte sectors ----------------
+			// The chunk finalised bins B0 .. B0+7 of block fl, B0 = k0 - G*fl - L - 1, which is not a multiple of 4:
+			// stored as they come, every 32-byte piece would straddle two sectors and leave both partially written,
+			// which DRAM has to complete by read-modify-write.  So each chunk writes the 8-bin aligned piece
+			// [A, A+8), A = B0 - r, r = B0 mod 8, whose last bin it has just finalised: bins A+i with i >= r come from
+			// this chunk's tile, bins A+i with i < r from the previous chunk's, which the lane kept in `carry`
+			// (tile index (i - r) & 7 in both cases).  A quarter-warp then stores one whole sector of each row.
+			// Every aligned piece ends in exactly one chunk, so every bin of [0, K) is written once (K is a multiple of
+			// 8: this kernel runs only at the paired FFT sizes, see chain_version()); the pieces of the first chunk only
+			// take carried bins below 0, which are masked.
+			// For L > 5 the carry's 32 registers would push the step into local memory: there r = 0, i.e. the finals
+			// are stored as they come (the presets have L = 3 or 4 at 48 kHz, 5 at 44.1 kHz).
 			{
+				constexpr bool ALIGN = LT <= 5;
 				float4 v[8];
-#pragma unroll
-				for (int it = 0; it < 8; ++it) v[it] = U.pvy[cb][fillI][fillF + 4 * it];
 #pragma unroll
 				for (int it = 0; it < 8; ++it) {
 					const int fl = fillF + 4 * it;
-					const int b = k0 + fillI - G * fl - LT - 1;
+					const int r = ALIGN ? (fl * (8 - (G & 7)) + 64 - LT - 1) & 7 : 0; // B0 mod 8 = (-G*fl - L - 1) mod 8
+					v[it] = U.pvy[cb][(fillI - r) & 7][fl];
+				}
+#pragma unroll
+				for (int it = 0; it < 8; ++it) {
+					const int fl = fillF + 4 * it;
+					const int r = ALIGN ? (fl * (8 - (G & 7)) + 64 - LT - 1) & 7 : 0;
+					const int b = k0 - G * fl - LT - 1 - r + fillI;
+					const float4 w = (!ALIGN || fillI >= r) ? v[it] : carry[it];
+					if constexpr (ALIGN) carry[it] = v[it];
 					if (fl < nAct && (unsigned)b < (unsigned)K) {
 						float2 *row = yBase + (size_t)(2 * fl) * K + b;
-						row[0] = make_float2(v[it].x, v[it].z);
-						row[K] = make_float2(v[it].y, v[it].w);
+						row[0] = make_float2(w.x, w.z);
+						row[K] = make_float2(w.y, w.w);
 					}
 				}
 			}
@@ -419,5 +440,8 @@ __global__ void __launch_bounds__(32) k_chain_direct4(Ctx x) {
 }
 
 static inline size_t smem_chain4(int) { return sizeof(Chain4Tiles); }
+// eight one-warp CTAs per SM (1024 streams on the 132 SMs of an H100 in one wave): the tiles, the 1 KB the system reserves
+// per CTA and at most 1 KB of static shared memory (tests/test_chain_resources.py checks the latter in the built library)
+static_assert(8 * (sizeof(Chain4Tiles) + 2048) <= 228 * 1024, "k_chain_direct4's tiles no longer fit eight CTAs per SM");
 
 } // namespace b200s

@@ -316,7 +316,8 @@ static int chain_version(const Cfg &g, int override, int forceFftV1) {
 	// default 4: the warp-specialised kernel (5) doubles the shared-memory traffic per step with its tile hand-off and its
 	// consumer waits for the producer
 	int want = override ? override : env ? env : 4;
-	if (want >= 3 && !(g.C == 2 && use_pair_fft(g, forceFftV1))) want = 2;
+	// (the packed stereo chains take whole 8-bin chunks of every row: K % CHAIN_CH == 0, true of both paired FFT sizes)
+	if (want >= 3 && !(g.C == 2 && use_pair_fft(g, forceFftV1) && g.K % CHAIN_CH == 0)) want = 2;
 	if (want == 5 && g.L > 4) want = 4; // k_chain_ws is laid out for L <= 4 (both presets)
 #ifndef B200S_KEEP_OLD_KERNELS
 	if (want == 1) want = 2;
