@@ -249,7 +249,28 @@ static bool use_pair_fft(const Cfg &g, int forceV1 = 0) {
 	if (v1 < 0) v1 = getenv("B200S_FFT_V1") ? 1 : 0; // A/B switch for profiling the first-generation kernels
 	return !v1 && !forceV1 && (g.K == 3072 || g.K == 2560);
 }
-static ChainKernel analyse2_kernel(const Cfg &g) { return g.K == 3072 ? k_analyse2<3072> : k_analyse2<2560>; }
+#ifdef B200S_ANALYSE_PROBES // profiling builds only: ablations of k_analyse2<3072> (wrong results), B200S_ANALYSE_PROBE=1..4
+static int analyse_probe() {
+	static int probe = -1;
+	if (probe < 0) {
+		const char *pv = getenv("B200S_ANALYSE_PROBE");
+		probe = pv ? atoi(pv) : 0;
+	}
+	return probe;
+}
+#endif
+static ChainKernel analyse2_kernel(const Cfg &g) {
+#ifdef B200S_ANALYSE_PROBES
+	if (g.K == 3072) switch (analyse_probe()) {
+		case 1: return k_analyse2<3072, 1>;
+		case 2: return k_analyse2<3072, 2>;
+		case 3: return k_analyse2<3072, 3>;
+		case 4: return k_analyse2<3072, 4>;
+		default: break;
+		}
+#endif
+	return g.K == 3072 ? k_analyse2<3072> : k_analyse2<2560>;
+}
 static ChainKernel synth2_kernel(const Cfg &g) { return g.K == 3072 ? k_synth2<3072> : k_synth2<2560>; }
 #ifdef B200S_KEEP_OLD_KERNELS
 static ChainKernel synth_kernel(const Cfg &g) { return g.K == 3072 ? k_synth<3072> : g.K == 2560 ? k_synth<2560> : k_synth<0>; }

@@ -15,7 +15,8 @@
 //     six shared-memory sweeps (the kernels were bound by shared-memory wavefronts and issue slots):
 //       - analysis: decimation in time.  The thread that windows and pre-twiddles its R3 input samples
 //         does the first (radix R3) butterfly on them in registers; the last radix-16 pass leaves the
-//         spectrum in registers in natural order and the caller stores it to HBM directly.
+//         spectrum in registers in natural order and the caller stores it (k_analyse2: back into the
+//         buffer in bin order, from where bulk copies take whole rows to HBM).
 //       - synthesis: decimation in frequency.  The first radix-16 pass takes its inputs from the caller
 //         (k_synth2 reads them from the spectra staged in the buffer); the last pass leaves the time samples
 //         in registers.

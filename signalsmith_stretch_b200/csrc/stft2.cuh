@@ -3,8 +3,9 @@
 //
 //   k_analyse2  windowed modified real FFT of TWO analyses at a time (dependency analyseStep,
 //               reference call sites signalsmith-stretch.h:337,359).  Persistent CTAs walk the
-//               (stream, job pair) items of the call; the raw samples of the NEXT pair are copied to
-//               shared memory with 16-byte cp.async while the current FFT runs.
+//               (stream, job pair) items of the call; the raw samples of the NEXT pair are bulk-copied to
+//               shared memory while the current FFT runs, and the spectrum rows leave the FFT buffer by
+//               bulk copies.
 //   k_synth2    inverse FFT of TWO consecutive blocks of one stream-channel at a time, synthesis
 //               window and overlap-add (synthesiseStep / readOutput / moveOutput, :397-414).  The two
 //               spectra of the NEXT pair are bulk-copied into the FFT buffer while the ring is updated;
@@ -32,11 +33,16 @@ __device__ __forceinline__ void st_stream(float *p, float v) { __stcs(p, v); }
 
 // ---------------------------------------------------------------------------------------------
 // k_analyse2: grid = persistent CTAs (a multiple of the SM count), 256 threads.
-// dyn smem: PairGeo::LEN float4 (FFT pair) + 2 * stage_len(B) floats (raw samples of the next pair).
+// dyn smem: PairGeo::LEN float4 (FFT pair; after the last pass it holds the pair's spectrum rows, stored by a bulk copy)
+// + 2 * stage_len(B) floats (raw samples of the next pair).
+// PROBE (profiling builds, -DB200S_ANALYSE_PROBES; wrong results on purpose) removes one part of the item to measure what
+// the kernel's time goes with: 1 the spectrum store, 2 the window / pre-twiddle table loads (a constant instead),
+// 3 the wait for the staged input (moved to just before the next copies are issued), 4 the FFT's stages B and C.
 // ---------------------------------------------------------------------------------------------
-template <int KT>
+template <int KT, int PROBE = 0>
 __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 	using G = PairGeo<KT>;
+	static_assert(2 * KT * sizeof(float2) <= G::LEN * sizeof(float4), "the spectrum rows of a pair fit the FFT buffer");
 	const Cfg &g = x.cfg;
 	B200S_DYN_SHARED
 	float4 *buf = (float4 *)dyn_smem;
@@ -135,15 +141,17 @@ __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 #endif
 			static_for<G::R3>([&](auto itc) {
 				constexpr int it = decltype(itc)::value;
-				tabr[it] = __ldg(x.anaTab + tid + 256 * it + wofs);
+				if constexpr (PROBE == 2) tabr[it] = make_float4(1.f, 1.f, 1.f, 0.f);
+				else tabr[it] = __ldg(x.anaTab + tid + 256 * it + wofs);
 			});
 		}
 		cp_async_wait_all();
-		if (x.inAligned) {
+		if (x.inAligned && PROBE != 3) {
 			mbar_wait(&stageBar, stagePar);
 			stagePar ^= 1u;
 		}
-		__syncthreads(); // staging complete and visible; previous unpack finished with buf
+		if (tid == 0) bulk_wait_read(); // the previous pair's spectrum has left buf
+		__syncthreads(); // staging complete and visible; buf free
 #ifdef B200S_EMU_EXACT_FFT // test builds only: swap in the oracle's double FFT to isolate the non-FFT logic
 		{
 			const int shA = x.inAligned ? (cur.a.start & 3) : 0, shB = x.inAligned ? (cur.b.start & 3) : 0;
@@ -196,33 +204,75 @@ __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 		Item n2;
 		long long cand = nitem + gridDim.x;
 		bool ok2 = false;
+		if constexpr (PROBE == 3) {
+			if (x.inAligned) {
+				mbar_wait(&stageBar, stagePar);
+				stagePar ^= 1u;
+			}
+		}
 		if (nitem < total) { // start the next pair's input on its way while this FFT runs
 			stage_job(stA, nxt.s, nxt.a, 0, 256);
 			stage_job(stB, nxt.s, nxt.b, 32, 256);
 			if (cand < total) fetch_raw(cand, n2); // descriptor of the item after next: loads in flight until the end of the iteration
 		}
-		pair_dit_stage_b<KT>(buf, tw, tid);
+		if constexpr (PROBE != 4) pair_dit_stage_b<KT>(buf, tw, tid);
 		__syncthreads();
-		if (tid < G::M1) { // ---- last pass fused with the store: thread holds X[tid + M1*q], q = 0..15.
-			// bin b = Z[b/2] (b even) or conj(Z[K-1-b/2]) (b odd): Z[k] with k < K/2 (q < 8) is bin 2k, the rest bin 2(K-1-k)+1
-			c2 v[16];
-			pair_dit_stage_c<KT>(buf, tw, tid, v);
-			const bool hasB = cur.hasB, il = x.specIl;
-			// stereo direct path: the pair is (channel 0, channel 1) of one analysis and is stored interleaved
-			float4 *dst4 = (float4 *)x.spec + ((size_t)cur.s * 2 * x.maxFrames + (cur.a.row >> 1)) * g.K;
-			static_for<16>([&](auto qc) {
-				constexpr int q = decltype(qc)::value;
-				const int k = tid + G::M1 * q;
-				const int b = q < 8 ? 2 * k : 2 * (KT - 1 - k) + 1;
-				const float sg = q < 8 ? 1.f : -1.f;
-				const float ra = f2_lo(v[q].re), rb = f2_hi(v[q].re), ia = sg * f2_lo(v[q].im), ib = sg * f2_hi(v[q].im);
-				if (il) {
-					dst4[b] = make_float4(ra, rb, ia, ib);
-				} else {
-					dstA[b] = make_float2(ra, ia);
-					if (hasB) dstB[b] = make_float2(rb, ib);
-				}
+		// ---- last pass: thread tid < M1 holds X[tid + M1*q], q = 0..15, in registers.
+		//      bin b = Z[b/2] (b even) or conj(Z[K-1-b/2]) (b odd): Z[k] with k < K/2 (q < 8) is bin 2k, the rest bin 2(K-1-k)+1.
+		//      The bins go back into buf in bin order and leave it as whole rows by bulk copies: stored from registers, each
+		//      warp instruction would write every other 16-byte half of its sectors (the other halves come from the mirror
+		//      warp), and two warps would sit idle through 96 store instructions per pair.
+		c2 v[16];
+		if (tid < G::M1) {
+			if constexpr (PROBE == 4) {
+				static_for<16>([&](auto qc) { v[decltype(qc)::value] = c2{f2_make((float)tid, 0.f), f2_make(0.f, (float)decltype(qc)::value)}; });
+			} else {
+				pair_dit_stage_c<KT>(buf, tw, tid, v);
+			}
+		} else {
+			// defined on the idle threads too: ptxas would otherwise keep all 64 registers live around the whole loop
+			static_for<16>([&](auto qc) { v[decltype(qc)::value] = c2{f2_make(0.f, 0.f), f2_make(0.f, 0.f)}; });
+		}
+		const bool hasB = cur.hasB, il = x.specIl;
+		if constexpr (PROBE == 1) {
+#ifndef B200S_EMU
+			if (tid < G::M1) static_for<16>([&](auto qc) {
+				const c2 w = v[decltype(qc)::value];
+				asm volatile("" ::"f"(w.re.a), "f"(w.re.b), "f"(w.im.a), "f"(w.im.b));
 			});
+#endif
+		} else {
+			__syncthreads(); // every read of buf has ended
+			if (tid < G::M1) {
+				// stereo direct path: the pair is (channel 0, channel 1) of one analysis, one row of float4 {re0, re1, im0, im1};
+				// otherwise row A at buf's first K float2, row B behind it
+				float2 *rowA = (float2 *)buf, *rowB = rowA + KT;
+				static_for<16>([&](auto qc) {
+					constexpr int q = decltype(qc)::value;
+					const int k = tid + G::M1 * q;
+					const int b = q < 8 ? 2 * k : 2 * (KT - 1 - k) + 1;
+					const float sg = q < 8 ? 1.f : -1.f;
+					const float ra = f2_lo(v[q].re), rb = f2_hi(v[q].re), ia = sg * f2_lo(v[q].im), ib = sg * f2_hi(v[q].im);
+					if (il) {
+						buf[b] = make_float4(ra, rb, ia, ib);
+					} else {
+						rowA[b] = make_float2(ra, ia);
+						rowB[b] = make_float2(rb, ib);
+					}
+				});
+			}
+			fence_async_proxy(); // the rows were written through the generic proxy; the bulk copies read them through the async one
+			__syncthreads();
+			if (tid == 0) {
+				constexpr unsigned row = (unsigned)sizeof(float2) * KT;
+				if (il) {
+					bulk_s2g((float4 *)x.spec + ((size_t)cur.s * 2 * x.maxFrames + (cur.a.row >> 1)) * g.K, buf, 2 * row);
+				} else {
+					bulk_s2g(dstA, buf, row);
+					if (hasB) bulk_s2g(dstB, (float2 *)buf + KT, row);
+				}
+				bulk_commit(); // waited for (source read) before the next pair's first pass writes buf
+			}
 		}
 		item = nitem;
 		cur = nxt;
@@ -233,6 +283,7 @@ __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 			nxt = n2;
 		}
 	}
+	if (tid == 0) bulk_wait_read(); // the shared memory of the last pair's rows stays allocated until they are read
 }
 
 // ---------------------------------------------------------------------------------------------
