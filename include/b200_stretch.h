@@ -84,16 +84,28 @@ int b200s_output_seek_length(const b200s_engine *e, float playback_rate);
 int b200s_fft_samples(const b200s_engine *e);
 int b200s_bands(const b200s_engine *e);
 
-/* ---- parameters, broadcast to every stream of the batch (:107-135) ---- */
+/* ---- parameters (:107-135).  Every stream has its own; these setters set every stream of the batch to the same value ---- */
 int b200s_set_transpose_factor(b200s_engine *e, float multiplier, float tonality_limit);
 int b200s_set_transpose_semitones(b200s_engine *e, float semitones, float tonality_limit);
 int b200s_set_formant_factor(b200s_engine *e, float multiplier, int compensate_pitch);
 int b200s_set_formant_semitones(b200s_engine *e, float semitones, int compensate_pitch);
 int b200s_set_formant_base(b200s_engine *e, float base_freq);
+/* The same setters per stream: arrays of `batch` entries, entry s set for stream s with the arithmetic of the setter above
+ * (so a stream is bit-identical to a one-stream engine given that stream's values).  tonality_limits / compensate_pitch
+ * may be NULL (0 for every stream).  Streams with different parameters run in one call: each stream takes the kernels
+ * its own parameters need (a server that transposes every user's stream by that user's amount, or the live wrapper's
+ * per-segment parameters, web/web-wrapper.js:233-235; signalsmith_stretch_b200/live.py). */
+int b200s_set_transpose_factor_per_stream(b200s_engine *e, const float *multipliers, const float *tonality_limits);
+int b200s_set_transpose_semitones_per_stream(b200s_engine *e, const float *semitones, const float *tonality_limits);
+int b200s_set_formant_factor_per_stream(b200s_engine *e, const float *multipliers, const int *compensate_pitch);
+int b200s_set_formant_semitones_per_stream(b200s_engine *e, const float *semitones, const int *compensate_pitch);
+int b200s_set_formant_base_per_stream(b200s_engine *e, const float *base_freqs);
 /* setFreqMap(std::function) (:120) cannot cross a C ABI (the reference's own wrapper says
  * "We can't do setFreqMap()", main.cpp:67).  The C++ facade tabulates the callable and passes a
  * monotone piecewise-linear map here: `n` points, freq_in[i] -> freq_out[i] (both as multiples
- * of the sample rate, freq_in ascending); linear extrapolation outside.  n == 0 clears it. */
+ * of the sample rate, freq_in ascending); linear extrapolation outside.  n == 0 clears it.
+ * One table per engine: it applies to every stream, until a transpose setter (broadcast or per stream) turns it off
+ * for every stream, as setTransposeFactor clears the reference's custom map. */
 int b200s_set_freq_map_table(b200s_engine *e, const float *freq_in, const float *freq_out, int n);
 
 /* ---- the hot path (:139-165 seek, :172-204 outputSeek, :209-423 process, :426-464 flush, :467-491 exact) ----

@@ -28,6 +28,8 @@ ABI_SYMBOLS = [
     "b200s_fft_samples", "b200s_bands",
     "b200s_set_transpose_factor", "b200s_set_transpose_semitones", "b200s_set_formant_factor",
     "b200s_set_formant_semitones", "b200s_set_formant_base", "b200s_set_freq_map_table",
+    "b200s_set_transpose_factor_per_stream", "b200s_set_transpose_semitones_per_stream", "b200s_set_formant_factor_per_stream",
+    "b200s_set_formant_semitones_per_stream", "b200s_set_formant_base_per_stream",
     "b200s_seek", "b200s_seek_rates", "b200s_live_seek", "b200s_output_seek", "b200s_process", "b200s_process_async", "b200s_process_pcm16", "b200s_flush", "b200s_exact",
     "b200s_seek_device", "b200s_process_device", "b200s_flush_device",
     "b200s_timer_start", "b200s_timer_stop", "b200s_kernel_launches", "b200s_device_allocations", "b200s_unserved_random_blocks", "b200s_profile_begin", "b200s_profile_end",
@@ -88,6 +90,9 @@ def _bind(lib):
         "b200s_set_transpose_factor": (ci, [vp, cf, cf]), "b200s_set_transpose_semitones": (ci, [vp, cf, cf]),
         "b200s_set_formant_factor": (ci, [vp, cf, ci]), "b200s_set_formant_semitones": (ci, [vp, cf, ci]),
         "b200s_set_formant_base": (ci, [vp, cf]), "b200s_set_freq_map_table": (ci, [vp, fp, fp, ci]),
+        "b200s_set_transpose_factor_per_stream": (ci, [vp, fp, fp]), "b200s_set_transpose_semitones_per_stream": (ci, [vp, fp, fp]),
+        "b200s_set_formant_factor_per_stream": (ci, [vp, fp, ip]), "b200s_set_formant_semitones_per_stream": (ci, [vp, fp, ip]),
+        "b200s_set_formant_base_per_stream": (ci, [vp, fp]),
         "b200s_seek": (ci, [vp, vp, ci, cd]), "b200s_seek_rates": (ci, [vp, vp, ci, ctypes.POINTER(cd)]), "b200s_live_seek": (ci, [vp, vp, cll, ctypes.POINTER(cll), ci, ctypes.POINTER(cd)]), "b200s_output_seek": (ci, [vp, vp, ci]),
         "b200s_process": (ci, [vp, vp, ci, vp, ci]), "b200s_process_async": (ci, [vp, vp, ci, vp, ci]), "b200s_process_pcm16": (ci, [vp, vp, ci, vp, ci, ci]), "b200s_flush": (ci, [vp, vp, ci, cf]),
         "b200s_exact": (ci, [vp, vp, ci, vp, ci, ip]),
@@ -204,21 +209,54 @@ class BatchStretch:
     def bands(self):
         return self._lib.b200s_bands(self._h)
 
-    # ---- parameters (:107-135) ----
+    # ---- parameters (:107-135): every argument is a scalar (broadcast to every stream) or one value per stream ----
+    def _per_stream(self, *args):
+        """args: (value, dtype) pairs.  None when every value is a scalar (the broadcast setter applies); otherwise every
+        value as a contiguous array of `batch` entries (a scalar is repeated), for the per-stream setter."""
+        if all(np.ndim(v) == 0 for v, _ in args):
+            return None
+        out = []
+        for v, dt in args:
+            a = np.ascontiguousarray(np.broadcast_to(np.asarray(v, dt), (self.batch,)) if np.ndim(v) == 0 else np.asarray(v, dt))
+            if a.shape != (self.batch,):
+                raise ValueError("expected a scalar or %d values (one per stream), got shape %s" % (self.batch, np.shape(v)))
+            out.append(a.ctypes.data_as(ctypes.POINTER(ctypes.c_int if dt == np.int32 else ctypes.c_float)))  # (keeps `a` alive)
+        return out
+
     def setTransposeFactor(self, multiplier, tonalityLimit=0.0):
-        self._ck(self._lib.b200s_set_transpose_factor(self._h, multiplier, tonalityLimit))
+        a = self._per_stream((multiplier, np.float32), (tonalityLimit, np.float32))
+        if a is None:
+            self._ck(self._lib.b200s_set_transpose_factor(self._h, multiplier, tonalityLimit))
+        else:
+            self._ck(self._lib.b200s_set_transpose_factor_per_stream(self._h, a[0], a[1]))
 
     def setTransposeSemitones(self, semitones, tonalityLimit=0.0):
-        self._ck(self._lib.b200s_set_transpose_semitones(self._h, semitones, tonalityLimit))
+        a = self._per_stream((semitones, np.float32), (tonalityLimit, np.float32))
+        if a is None:
+            self._ck(self._lib.b200s_set_transpose_semitones(self._h, semitones, tonalityLimit))
+        else:
+            self._ck(self._lib.b200s_set_transpose_semitones_per_stream(self._h, a[0], a[1]))
 
     def setFormantFactor(self, multiplier, compensatePitch=False):
-        self._ck(self._lib.b200s_set_formant_factor(self._h, multiplier, int(compensatePitch)))
+        a = self._per_stream((multiplier, np.float32), (compensatePitch, np.int32))
+        if a is None:
+            self._ck(self._lib.b200s_set_formant_factor(self._h, multiplier, int(compensatePitch)))
+        else:
+            self._ck(self._lib.b200s_set_formant_factor_per_stream(self._h, a[0], a[1]))
 
     def setFormantSemitones(self, semitones, compensatePitch=False):
-        self._ck(self._lib.b200s_set_formant_semitones(self._h, semitones, int(compensatePitch)))
+        a = self._per_stream((semitones, np.float32), (compensatePitch, np.int32))
+        if a is None:
+            self._ck(self._lib.b200s_set_formant_semitones(self._h, semitones, int(compensatePitch)))
+        else:
+            self._ck(self._lib.b200s_set_formant_semitones_per_stream(self._h, a[0], a[1]))
 
     def setFormantBase(self, baseFreq=0.0):
-        self._ck(self._lib.b200s_set_formant_base(self._h, baseFreq))
+        a = self._per_stream((baseFreq, np.float32))
+        if a is None:
+            self._ck(self._lib.b200s_set_formant_base(self._h, baseFreq))
+        else:
+            self._ck(self._lib.b200s_set_formant_base_per_stream(self._h, a[0]))
 
     def setFreqMap(self, inputToOutput, points=2049):
         """setFreqMap(std::function) (:120): the callable is tabulated on [0, 0.5] (piecewise linear)."""

@@ -41,7 +41,7 @@ __global__ void __launch_bounds__(32) k_chain_direct(Ctx x) {
 	if (s >= x.sBase + x.sCount) return;
 	const Call cl = x.call[s];
 	if (cl.nFrames == 0) return;
-	if (cl.hasRandom && x.randomPathOn) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
+	if (cl.mapped || (cl.hasRandom && x.randomPathOn)) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
 	constexpr int D = LT + 1;
 	DirectTiles2<CT> &U = ((DirectTiles2<CT> *)dyn_smem)[warp];
 	const int fillI = lane & 7, fillF = lane >> 3;

@@ -72,6 +72,7 @@ __device__ __forceinline__ bool dual_pair_ok(const Ctx &x, int s, int lane) {
 	const Call a = x.call[s], b = x.call[s + 1];
 	if (a.nFrames == 0 || a.nFrames != b.nFrames || a.bypass || b.bypass) return false;
 	if ((a.hasRandom || b.hasRandom) && x.randomPathOn) return false;
+	if (a.mapped || b.mapped) return false; // a partner on the mapped path: the plain stream runs alone
 	bool bad = false;
 	for (int f = lane; f < a.nFrames; f += 32) {
 		const Frame fa = x.frames[(size_t)s * x.maxFrames + f], fb = x.frames[(size_t)(s + 1) * x.maxFrames + f];
@@ -93,7 +94,7 @@ __global__ void __launch_bounds__(32 * CH2_MAXW) k_chain_direct2(Ctx x) {
 	const int j = lane / CT, c = lane % CT; // block within the warp, channel
 	const int s = x.sBase + blockIdx.x;
 	const Call cl = x.call[s];
-	if (cl.nFrames == 0) return;
+	if (cl.nFrames == 0 || cl.mapped) return; // (streams with a frequency map or formants: the mapped path)
 	if (cl.hasRandom && x.randomPathOn) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
 	Chain2Sync &SY = *(Chain2Sync *)dyn_smem;
 	Chain2Tiles<CT> &U = ((Chain2Tiles<CT> *)((char *)dyn_smem + 64))[warp];

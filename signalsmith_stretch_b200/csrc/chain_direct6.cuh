@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(32) k_chain_direct6(Ctx x) {
 	for (int pass = 0; pass < nPass; ++pass) {
 	const int s = s0 + pass;
 	const Call cl = x.call[s];
-	if (cl.nFrames == 0) continue;
+	if (cl.nFrames == 0 || cl.mapped) continue; // (streams with a frequency map or formants: the mapped path)
 	if (cl.hasRandom && x.randomPathOn) continue; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
 	const int sH[2] = {s, pairOk ? s + 1 : s};
 	for (int base = 0; base < cl.nFrames; base += 32) {

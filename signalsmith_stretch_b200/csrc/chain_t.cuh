@@ -29,13 +29,13 @@ __device__ __forceinline__ size_t t_idx(const Ctx &x, int s, int grp, int k, int
 
 __global__ void __launch_bounds__(256) k_products(Ctx x) {
 	const Cfg &g = x.cfg;
-	const Params &prm = x.prm;
 	const int K = g.K, LT = g.L, D = LT + 1;
 	const int k0 = blockIdx.x * 32, grp = blockIdx.y, s = x.sBase + blockIdx.z;
 	const int i = threadIdx.x & 31, w = threadIdx.x >> 5;
 	const Call cl = x.call[s];
 	const int base = 32 * grp, nAct = min(32, cl.nFrames - base);
-	if (cl.bypass || nAct <= 0 || (cl.hasRandom && x.randomPathOn)) return;
+	// (plain streams of a mixed call: the direct chain writes their Y rows)
+	if (cl.bypass || nAct <= 0 || !cl.mapped || (cl.hasRandom && x.randomPathOn)) return;
 	B200S_SHARED float2 tFT[32][33], tT2[32][33], tT1[32][33], tPI[32][33];
 	B200S_SHARED float tE[32][33];
 	for (int c = 0; c < g.C; ++c) {
@@ -124,6 +124,9 @@ __global__ void __launch_bounds__(32) k_chain_t(Ctx x) {
 	const int K = g.K;
 	const int lane = threadIdx.x & 31;
 	const int s = x.sBase + blockIdx.x;
+	// plain streams of a mixed call: the direct chain.  (A separate read-only load: testing the field of `cl` below costs the
+	// L = 8 stereo instantiation 60 more bytes of spills.)
+	if (!__ldg(&x.call[s].mapped)) return;
 	const Call cl = x.call[s];
 	if (cl.nFrames == 0) return;
 	if (cl.hasRandom && x.randomPathOn) return; // random time factors: k_prep + k_chain take the stream

@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(64, 7) k_chain_ws(Ctx x) {
 	const int s = x.sBase + blockIdx.x;
 	const Call cl = x.call[s];
 	if (cl.nFrames == 0) return;
-	if (cl.hasRandom && x.randomPathOn) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
+	if (cl.mapped || (cl.hasRandom && x.randomPathOn)) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
 	if (!ws_stream_ok(x, s, cl.nFrames, lane)) return; // k_chain_direct4 takes this stream
 	WsTiles<FAST> &U = *(WsTiles<FAST> *)dyn_smem;
 	const float one = x.one; // unused by the f2 arithmetic (see padd / psub)

@@ -55,7 +55,8 @@ struct Cfg {
 	int radix[20];
 };
 
-// user parameters (:107-135), broadcast to every stream
+// user parameters (:107-135) of one stream in the form map_freq / inv_map_formant take: built by stream_params from the
+// stream's entry of Ctx::sprm and the engine's frequency map table Ctx::fmap
 struct Params {
 	float freqMultiplier, freqTonalityLimit;
 	float formantMultiplier, invFormantMultiplier, formantBaseFreq;
@@ -63,6 +64,23 @@ struct Params {
 	int mapN;                 // >0: custom piecewise-linear frequency map (setFreqMap, :120)
 	const float *mapIn, *mapOut;
 };
+
+// the custom frequency map table (setFreqMap, :120): one per engine
+struct FreqMap {
+	int mapN; // >0: piecewise-linear map of mapN points
+	const float *mapIn, *mapOut;
+};
+
+// the parameters of one stream (b200s_set_*_per_stream; the broadcast setters write every entry)
+struct StreamParams {
+	float freqMultiplier, freqTonalityLimit;
+	float formantMultiplier, invFormantMultiplier, formantBaseFreq;
+	int formantCompensation;
+	int customMap; // the stream uses the engine's frequency map table (set by b200s_set_freq_map_table, cleared by a transpose setter)
+};
+// which path a stream's parameters need: frequency map (:300) and formant processing (:310); neither = pure time-stretch
+__host__ __device__ __forceinline__ bool stream_mapped(const StreamParams &p, int mapN) { return (p.customMap && mapN > 0) || p.freqMultiplier != 1.0f; }
+__host__ __device__ __forceinline__ bool stream_formants(const StreamParams &p, bool mapped) { return p.formantMultiplier != 1.0f || (p.formantCompensation && mapped); }
 
 // per-stream block scheduler state (:494-529)
 struct Sched {
@@ -92,6 +110,8 @@ struct Call {
 	int finalIn, finalPrev; // slots that become stIn / stPrev after the call
 	int nJobs;              // analyses of this call (entries of the stream's Job list)
 	int hasRandom;          // some block of the call stretches beyond 2x (:639): the stream takes the k_prep + k_chain path
+	int mapped;             // the stream's parameters need a frequency map or formants: mapped-path kernels, planar spectra
+	int autoPitch;          // formants with the automatic pitch estimate (formant base <= 0): k_pitch takes the stream
 };
 
 // one windowed analysis FFT of the call (:333-376): block samples start at stream index `start`
@@ -103,7 +123,8 @@ struct Job {
 // everything a kernel needs, passed by value
 struct Ctx {
 	Cfg cfg;
-	Params prm;
+	FreqMap fmap;
+	const StreamParams *sprm; // [S] per-stream parameters
 	// tables
 	const float *window, *winProd, *wpReset;
 	const float2 *rot, *twiddle, *pretw;
@@ -117,7 +138,8 @@ struct Ctx {
 	float *stPredE;
 	float *stPitch; // [S][2] freqEstimateWeighted, freqEstimateWeight (:927-928): automatic pitch estimate of the formant envelope
 	// stereo direct path: spectra are channel-interleaved float4 {re0, re1, im0, im1} per bin (chain_direct3.cuh);
-	// stIl [S][2][K] holds such copies of stIn / stPrev, made by k_plan at the start of the call
+	// stIl [S][2][K] holds such copies of stIn / stPrev, made by k_plan at the start of the call.  Per stream: the
+	// streams with Call::mapped keep planar rows (spec_il)
 	float4 *stIl;
 	int specIl;
 	int wsRan; // k_chain_ws ran before k_chain_direct4 in this call: the latter only takes the streams the former left (chain_ws.cuh)

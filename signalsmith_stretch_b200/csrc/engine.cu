@@ -7,6 +7,8 @@
 //                                                  -> k_synth2 || k_commit (side stream)
 //   mapped / formants:  k_plan -> k_analyse2 -> [k_pitch] -> k_energy -> k_passes -> k_prep (map-only) -> k_products
 //                       -> k_chain_t -> k_synth2 || k_commit                                        (chain_t.cuh)
+//   the path is decided per stream from its own parameters (Call::mapped): a call whose streams differ launches both
+//   sequences, and each kernel exits at once for the streams of the other path
 //   calls that may stretch beyond 2x additionally launch k_prep + k_chain in random-only mode: they take the streams
 //   whose blocks draw random time factors (Call::hasRandom, decided per stream by k_plan); every other CTA exits at once
 //   generic sizes (not 3072 / 2560 bands): k_analyse / k_synth (fft.cuh), k_chain_direct2 (plain) / k_chain (mapped)
@@ -42,7 +44,19 @@ struct b200s_engine {
 	long seed = 0;
 	bool configured = false;
 	Cfg cfg;
-	Params prm;
+	FreqMap fmap; // the custom frequency map table (mapN; its device rows are dMapIn / dMapOut)
+	// per-stream parameters: the host table (what the setters write) and its device copy Ctx::sprm, uploaded by the next
+	// process() when dirty; the counts over the table decide which kernels a call launches
+	std::vector<StreamParams> hSprm;
+	StreamParams *dSprm = 0;
+	bool sprmDirty = true;
+	// pinned staging of the upload, two copies: an asynchronous call returns once enqueued (from pageable memory the copy
+	// could wait for the queued work); a copy is rewritten once the upload issued from it two uploads ago has run
+	StreamParams *pinSprm[2] = {0, 0};
+	cudaEvent_t evSprm[2] = {0, 0};
+	int sprmSlot = 0;
+	int nMapped = 0;                              // streams on the mapped / formant path (Call::mapped)
+	bool anyFormants = false, anyAutoPitch = false; // some stream processes formants / with the automatic pitch estimate
 	cudaStream_t stream = 0;
 	bool ownStream = false;
 	// sub-batch pipeline: process() splits the batch over these prioritised streams (see process_impl)
@@ -153,6 +167,23 @@ static void dfree(T *&p) {
 	p = 0;
 }
 
+// page-locked host memory (the CPU emulator of the tests has none: plain memory there)
+static bool host_alloc(void **p, size_t bytes) {
+#ifdef B200S_EMU
+	*p = malloc(bytes);
+	return *p != 0;
+#else
+	return cudaMallocHost(p, bytes) == cudaSuccess;
+#endif
+}
+static void host_free(void *p) {
+#ifdef B200S_EMU
+	free(p);
+#else
+	if (p) cudaFreeHost(p);
+#endif
+}
+
 static void free_all(b200s_engine *e) {
 	dfree(e->dWindow); dfree(e->dWinProd); dfree(e->dWpReset); dfree(e->dRot); dfree(e->dTwiddle); dfree(e->dPretw); dfree(e->dAnaTab);
 	dfree(e->dSched); dfree(e->dHist[0]); dfree(e->dHist[1]); dfree(e->dPend); dfree(e->dPendWp);
@@ -170,9 +201,10 @@ static Ctx make_ctx(b200s_engine *e) {
 	Ctx x;
 	memset(&x, 0, sizeof(x));
 	x.cfg = e->cfg;
-	x.prm = e->prm;
-	x.prm.mapIn = e->dMapIn;
-	x.prm.mapOut = e->dMapOut;
+	x.fmap.mapN = e->fmap.mapN;
+	x.fmap.mapIn = e->dMapIn;
+	x.fmap.mapOut = e->dMapOut;
+	x.sprm = e->dSprm;
 	x.window = e->dWindow; x.winProd = e->dWinProd; x.wpReset = e->dWpReset;
 	x.rot = e->dRot; x.twiddle = e->dTwiddle; x.pretw = e->dPretw; x.anaTab = e->dAnaTab;
 	x.rot0 = e->rot0; x.rotStep = e->rotStep;
@@ -259,7 +291,9 @@ static int analyse_probe() {
 	return probe;
 }
 #endif
-static ChainKernel analyse2_kernel(const Cfg &g) {
+// mixed: a stereo call with interleaved rows for its plain streams and planar rows for its mapped ones (§3.9 of DESIGN.md)
+static ChainKernel analyse2_kernel(const Cfg &g, bool mixed = false) {
+	if (mixed) return g.K == 3072 ? k_analyse2_mixed<3072> : k_analyse2_mixed<2560>;
 #ifdef B200S_ANALYSE_PROBES
 	if (g.K == 3072) switch (analyse_probe()) {
 		case 1: return k_analyse2<3072, 1>;
@@ -614,6 +648,11 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 		}
 	}
 
+	if (!e->dSprm) { // the per-stream parameter table (kept over configure, like the parameters themselves)
+		if ((rc = dalloc(e, &e->dSprm, (size_t)g.S))) return rc;
+		e->sprmDirty = true;
+	}
+
 	// ---- state
 	const size_t SC = (size_t)g.S * g.C;
 	if ((rc = dalloc(e, &e->dSched, g.S))) return rc;
@@ -667,6 +706,7 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 	CK(cudaFuncSetAttribute(g.C == 1 ? chain6_kernel<false, true>(g.L) : chain6_kernel<false, false>(g.L), cudaFuncAttributePreferredSharedMemoryCarveout, 100));
 	if (use_pair_fft(g)) {
 		CK(cudaFuncSetAttribute(analyse2_kernel(g), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_analyse2(g)));
+		CK(cudaFuncSetAttribute(analyse2_kernel(g, true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_analyse2(g)));
 		CK(cudaFuncSetAttribute(synth2_kernel(g), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_synth2(g)));
 	}
 	{
@@ -700,12 +740,24 @@ static int ensure_scratch(b200s_engine *e, int nOut) {
 	e->coefFrames = e->randFrames = e->tFrames = 0;
 	return 0;
 }
-// Complex coefficient rows of k_prep (32 B per bin-channel and block: 6.6 GB at batch 1024 x 33 blocks stereo): only calls
-// with a frequency map or formant processing launch k_prep, so only they pay for them (b200s_reserve() allocates them
-// when the parameters set at that time need them).
-static bool params_plain(const b200s_engine *e) {
-	return !(e->prm.mapN > 0 || e->prm.freqMultiplier != 1.0f) && e->prm.formantMultiplier == 1.0f;
+// The counts over the per-stream table that decide a call's kernels (k_plan decides each stream's path by the same test)
+static void count_paths(b200s_engine *e) {
+	e->nMapped = 0;
+	e->anyFormants = e->anyAutoPitch = false;
+	for (const StreamParams &p : e->hSprm) {
+		const bool mapped = stream_mapped(p, e->fmap.mapN), formants = stream_formants(p, mapped);
+		e->nMapped += (mapped || formants) ? 1 : 0;
+		e->anyFormants = e->anyFormants || formants;
+		e->anyAutoPitch = e->anyAutoPitch || (formants && !(p.formantBaseFreq > 0));
+	}
 }
+static void params_changed(b200s_engine *e) {
+	count_paths(e);
+	e->sprmDirty = true;
+}
+// Complex coefficient rows of k_prep (32 B per bin-channel and block: 6.6 GB at batch 1024 x 33 blocks stereo): only calls
+// with a stream that has a frequency map or formant processing launch k_prep, so only they pay for them (b200s_reserve()
+// allocates them when the parameters set at that time need them).
 static int ensure_coef(b200s_engine *e) {
 	if (e->coefFrames == e->maxFrames && e->dPI) return 0;
 	const Cfg &g = e->cfg;
@@ -778,6 +830,18 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	}
 	int rc;
 	if ((rc = ensure_scratch(e, nOut))) return rc;
+	if (e->sprmDirty) {
+		// new per-stream parameters, on the main stream ahead of this call's work.  This call then joins (see `chained`
+		// below): a chained call's stream groups do not wait for the main stream, so they could read the new table while
+		// the previous call's groups are still running.
+		const int k = e->sprmSlot ^= 1;
+		CK(cudaEventSynchronize(e->evSprm[k]));
+		memcpy(e->pinSprm[k], e->hSprm.data(), sizeof(StreamParams) * e->S);
+		CK(cudaMemcpyAsync(e->dSprm, e->pinSprm[k], sizeof(StreamParams) * e->S, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaEventRecord(e->evSprm[k], e->stream));
+		e->sprmDirty = false;
+		e->chainedGroups = 0;
+	}
 	// Can a block of this call stretch beyond 2x (timeFactor = interval / inputInterval > 2, :312,:639)?  Inside a call the
 	// input interval is interval * nIn / nOut give or take a sample; the first block's mixes in the previous call's ratio;
 	// after a seek it is 1 / playbackRate.  Conservative on purpose: the decision itself is taken per stream on the device
@@ -788,13 +852,17 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 		e->prevCallMayRandom = lowRatio;
 		e->seekMayRandom = false;
 	}
-	const bool useStepMajor = !params_plain(e) && e->stepMajor; // mapped / formant call on k_products + k_chain_t
-	if (((!params_plain(e) && !useStepMajor) || mayRandom) && (rc = ensure_coef(e))) return rc;
+	// Each stream takes the path its own parameters need (k_plan sets Call::mapped); a call launches the kernels of the paths
+	// some stream takes, and every kernel skips the streams of the other path.  With the same parameters on every stream
+	// this is one of the two uniform launch sequences.
+	const bool anyMapped = e->nMapped > 0, anyPlain = e->nMapped < e->S;
+	const bool useStepMajor = anyMapped && e->stepMajor; // mapped / formant streams on k_products + k_chain_t
+	if (((anyMapped && !useStepMajor) || mayRandom) && (rc = ensure_coef(e))) return rc;
 	if (useStepMajor && (rc = ensure_stepmajor(e))) return rc;
 	if (mayRandom && (rc = ensure_rand(e))) return rc;
 	Ctx x = make_ctx(e);
 	if (!mayRandom) x.cT1u = x.cT2u = nullptr; // (stale rows of an earlier call are never read)
-	x.randomPathOn = (mayRandom || (!params_plain(e) && !useStepMajor)) ? 1 : 0; // the round-1 mapped path runs k_prep + k_chain for every stream anyway
+	x.randomPathOn = (mayRandom || (anyMapped && !useStepMajor)) ? 1 : 0; // the round-1 mapped path runs k_prep + k_chain for every random stream anyway
 	x.in = dIn; x.out = dOut; x.nIn = nIn; x.nOut = nOut;
 	x.inChanStride = inChanStride; x.inStreamStride = inStreamStride;
 	x.outChanStride = outChanStride; x.outStreamStride = outStreamStride;
@@ -822,11 +890,9 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	e->chainedIn = nIn;
 	e->chainedOut = nOut;
 	if (nSub > 1 && !chained) CK(cudaEventRecord(e->evBegin, e->stream));
-	const bool plain = params_plain(e);
-	const bool formantsOn = e->prm.formantMultiplier != 1.0f || (e->prm.formantCompensation && (e->prm.mapN > 0 || e->prm.freqMultiplier != 1.0f)); // :310
 	const int chainV = chain_version(g, e->chainV, e->fftV1);
 	const bool pairFft = use_pair_fft(g, e->fftV1);
-	x.specIl = (plain && chainV >= 3) ? 1 : 0;
+	x.specIl = (anyPlain && chainV >= 3) ? 1 : 0; // (interleaved rows for the plain streams only, spec_il)
 	for (int sub = 0; sub < nSub; ++sub) {
 		cudaStream_t st = nSub > 1 ? e->subStream[sub] : e->stream;
 		if (nSub > 1 && !chained) CK(cudaStreamWaitEvent(st, e->evBegin, 0));
@@ -846,7 +912,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 				if (pairFft) { // persistent CTAs, two per SM, over the (stream, job pair) items
 					const long long items = (long long)x.sCount * g.C * x.maxFrames;
 					const int grid = (int)std::min<long long>(items, 2LL * e->numSMs);
-					PROF(PK_ANALYSE, B200S_LAUNCH(analyse2_kernel(g), dim3(grid), dim3(256), smem_analyse2(g), st, x));
+					PROF(PK_ANALYSE, B200S_LAUNCH(analyse2_kernel(g, x.specIl && anyMapped), dim3(grid), dim3(256), smem_analyse2(g), st, x));
 				} else {
 					ChainKernel ka = analyse_kernel(g);
 					PROF(PK_ANALYSE, B200S_LAUNCH(ka, dim3(std::min(2 * F * g.C, ANALYSE_CTAS_PER_STREAM), 1, x.sCount), dim3(kThreads), smem_analyse(g), st, x));
@@ -854,11 +920,11 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 				// Pure time-stretch (no frequency map, no formants): the chain forms its terms directly from
 				// the spectra and k_prep is skipped; otherwise k_prep produces the coefficient arrays.
 				// formants with setFormantBase(0): the automatic pitch estimate of every block (serial over blocks) first
-				if (!plain && formantsOn && !(e->prm.formantBaseFreq > 0)) {
+				if (e->anyAutoPitch) {
 					B200S_LAUNCH(k_pitch, dim3(x.sCount), dim3(kThreads), sizeof(float) * g.K, st, x);
 					CKL();
 				}
-				if (!plain) {
+				if (anyMapped) {
 					int _rc;
 					if ((_rc = prof_mark(e, PK_PREP, true))) return _rc;
 					// the serial one-pole passes over the bins, one lane per block (kernels.cuh), then the per-bin products
@@ -868,30 +934,32 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 					CKL();
 					if (useStepMajor) { // peaks / map / ratio rows, then the per-bin terms in step-major order (chain_t.cuh)
 						x.mapOnly = 1;
-						B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, formantsOn), st, x);
+						B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, e->anyFormants), st, x);
 						CKL();
 						x.mapOnly = 0;
 						B200S_LAUNCH(k_products, dim3(x.tRows / 32, x.tGroups, x.sCount), dim3(256), 0, st, x);
 						CKL();
-						if (mayRandom) { // streams with a random block: the full k_prep (random-only mode), consumed by k_chain below
+						if (mayRandom) { // streams with a random block (plain or mapped): the full k_prep (random-only mode), consumed by k_chain below
 							x.randomOnly = 1;
-							B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, formantsOn), st, x);
+							B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, e->anyFormants), st, x);
 							CKL();
 							x.randomOnly = 0;
 						}
 					} else {
-						B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, formantsOn), st, x);
+						B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, e->anyFormants), st, x);
 						CKL();
 					}
 					if ((_rc = prof_mark(e, PK_PREP, false))) return _rc;
 				}
+				// the mapped / formant streams (k_chain_t, or the round-1 k_chain), then the plain streams (a direct chain); in a
+				// mixed call each of these kernels exits at once for the other path's streams
 				if (useStepMajor) {
 					int _rc;
 					if ((_rc = prof_mark(e, PK_CHAIN, true))) return _rc;
 					ChainKernel kt = chain_t_kernel(g);
 					B200S_LAUNCH(kt, dim3(x.sCount), dim3(32), 0, st, x);
 					CKL();
-					if (mayRandom) { // the streams k_chain_t left (Call::hasRandom)
+					if (mayRandom) { // the streams k_chain_t and the direct chains leave (Call::hasRandom), plain or mapped
 						x.randomOnly = 1;
 						dim3 grid((x.sCount + kChainWarps - 1) / kChainWarps), block(32 * kChainWarps);
 						ChainKernel kc = chain_kernel(g, false);
@@ -900,8 +968,14 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 						x.randomOnly = 0;
 					}
 					if ((_rc = prof_mark(e, PK_CHAIN, false))) return _rc;
+				} else if (anyMapped) { // round-1 kernels: the mapped streams and every stream with a random block
+					dim3 grid((x.sCount + kChainWarps - 1) / kChainWarps), block(32 * kChainWarps);
+					ChainKernel kc = chain_kernel(g, false);
+					PROF(PK_CHAIN, B200S_LAUNCH(kc, grid, block, smem_chain(g, false, mayRandom), st, x));
+				}
+				if (!anyPlain) {
 #ifdef B200S_KEEP_OLD_KERNELS
-				} else if (plain && chainV == 5) {
+				} else if (chainV == 5) {
 					int _rc;
 					if ((_rc = prof_mark(e, PK_CHAIN, true))) return _rc;
 					const bool fast = !e->exactMath;
@@ -914,9 +988,9 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 					x.wsRan = 0;
 					if ((_rc = prof_mark(e, PK_CHAIN, false))) return _rc;
 #endif
-				} else if (plain && chainV >= 3) {
+				} else if (chainV >= 3) {
 					PROF(PK_CHAIN, B200S_LAUNCH(chain3_kernel(g, chainV, !e->exactMath), dim3(x.sCount), dim3(32), chainV >= 6 ? smem_chain6() : chainV == 4 ? smem_chain4(g.L) : sizeof(Chain3Tiles), st, x));
-				} else if (plain && chainV == 2) {
+				} else if (chainV == 2) {
 					const int W = chain2_warps(g, nOut);
 					ChainKernel kc = chain2_kernel(g, g.C == 1 && !e->exactMath);
 					int _rc;
@@ -929,16 +1003,17 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 					}
 					CKL();
 					if ((_rc = prof_mark(e, PK_CHAIN, false))) return _rc;
-				} else {
+				} else { // (first-generation direct chain, -DB200S_KEEP_OLD_KERNELS builds only)
 					dim3 grid((x.sCount + kChainWarps - 1) / kChainWarps), block(32 * kChainWarps);
-					ChainKernel kc = chain_kernel(g, plain);
-					PROF(PK_CHAIN, B200S_LAUNCH(kc, grid, block, smem_chain(g, plain, mayRandom), st, x));
+					ChainKernel kc = chain_kernel(g, true);
+					PROF(PK_CHAIN, B200S_LAUNCH(kc, grid, block, smem_chain(g, true, mayRandom), st, x));
 				}
 			}
-			if (F > 0 && plain && mayRandom) {
+			if (F > 0 && !anyMapped && mayRandom) {
 				// streams with a block beyond 2x stretch (Call::hasRandom): the direct chain kernels above returned at once for
 				// them; k_prep forms their coefficient rows with the per-bin random time factors and the generic chain runs
-				// them.  Every other CTA of these two launches exits immediately.
+				// them.  Every other CTA of these two launches exits immediately.  (Calls with mapped streams have run these
+				// streams on the mapped path's random-only launches above.)
 				x.randomOnly = 1;
 				B200S_LAUNCH(k_prep, dim3(F, x.sCount), dim3(kThreads), smem_prep(g, false), st, x);
 				CKL();
@@ -1095,10 +1170,16 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 	e->seed = seed;
 	e->device = device;
 	memset(&e->cfg, 0, sizeof(e->cfg));
-	memset(&e->prm, 0, sizeof(e->prm));
-	e->prm.freqMultiplier = 1;
-	e->prm.freqTonalityLimit = 0.5f; // :513
-	e->prm.formantMultiplier = e->prm.invFormantMultiplier = 1;
+	memset(&e->fmap, 0, sizeof(e->fmap));
+	{
+		StreamParams p;
+		memset(&p, 0, sizeof(p));
+		p.freqMultiplier = 1;
+		p.freqTonalityLimit = 0.5f; // :513
+		p.formantMultiplier = p.invFormantMultiplier = 1;
+		e->hSprm.assign((size_t)batch, p);
+		params_changed(e);
+	}
 	if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess ||
 	    cudaEventCreate(&e->evStart) != cudaSuccess || cudaEventCreate(&e->evStop) != cudaSuccess) {
 		g_createError = "CUDA stream/event creation failed";
@@ -1114,6 +1195,13 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 		    cudaEventCreateWithFlags(&e->evJoin, cudaEventDisableTiming) != cudaSuccess)
 			e->commitStream = 0; // (no fork then: the commit follows the synthesis on the main stream)
 	}
+	for (int k = 0; k < 2; ++k)
+		if (!host_alloc((void **)&e->pinSprm[k], sizeof(StreamParams) * (size_t)batch) ||
+		    cudaEventCreateWithFlags(&e->evSprm[k], cudaEventDisableTiming) != cudaSuccess) {
+			g_createError = "pinned host memory / event creation failed";
+			b200s_destroy(e);
+			return B200S_ECUDA;
+		}
 	{ // sub-batch streams: highest priority first
 		int lo = 0, hi = 0;
 		cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -1145,6 +1233,11 @@ void b200s_destroy(b200s_engine *e) {
 	dfree(e->dDiag);
 	dfree(e->dSeekStf);
 	dfree(e->dSeekEnd);
+	dfree(e->dSprm);
+	for (int k = 0; k < 2; ++k) {
+		host_free(e->pinSprm[k]);
+		if (e->evSprm[k]) cudaEventDestroy(e->evSprm[k]);
+	}
 	for (int i = 0; i < b200s_engine::kMaxSub; ++i) {
 		if (e->subStream[i]) cudaStreamDestroy(e->subStream[i]);
 		if (e->evSubDone[i]) cudaEventDestroy(e->evSubDone[i]);
@@ -1221,7 +1314,7 @@ int b200s_reserve(b200s_engine *e, int maxIn, int maxOut) {
 	NEED_CFG();
 	int rc;
 	if ((rc = ensure_scratch(e, maxOut))) return rc;
-	if (!params_plain(e) && (rc = e->stepMajor ? ensure_stepmajor(e) : ensure_coef(e))) return rc;
+	if (e->nMapped > 0 && (rc = e->stepMajor ? ensure_stepmajor(e) : ensure_coef(e))) return rc;
 	if ((rc = stage_in(e, 0, 0))) return rc;
 	size_t ci = (size_t)e->cfg.S * e->cfg.C * std::max(maxIn, 1), co = (size_t)e->cfg.S * e->cfg.C * std::max(maxOut, 1);
 	if ((rc = ensure_buf(e, &e->dIn, &e->inCap, ci, false))) return rc;
@@ -1242,30 +1335,73 @@ int b200s_output_seek_length(const b200s_engine *e, float rate) {               
 int b200s_fft_samples(const b200s_engine *e) { return e && e->configured ? e->cfg.N : 0; }
 int b200s_bands(const b200s_engine *e) { return e && e->configured ? e->cfg.K : 0; }
 
-int b200s_set_transpose_factor(b200s_engine *e, float multiplier, float tonality) { // :107-115
+// One stream's entry, set by exactly the arithmetic of the reference's setters: the broadcast setters apply these to every
+// entry, the per-stream ones entry by entry, so a stream gets the same bits either way (and as a one-stream reference).
+static void set_transpose(StreamParams &p, float multiplier, float tonality) { // :107-115
+	p.freqMultiplier = multiplier;
+	if (tonality > 0) p.freqTonalityLimit = tonality / std::sqrt(multiplier);
+	else p.freqTonalityLimit = 1;
+	p.customMap = 0; // (setTransposeFactor clears customFreqMap)
+}
+static float semitones_factor(float semitones) { return std::pow(2, semitones / 12); } // :116-118, :129-131
+static void set_formant(StreamParams &p, float multiplier, int comp) { // :124-128
+	p.formantMultiplier = multiplier;
+	p.invFormantMultiplier = 1 / multiplier;
+	p.formantCompensation = comp ? 1 : 0;
+}
+
+int b200s_set_transpose_factor(b200s_engine *e, float multiplier, float tonality) {
 	if (!e) return B200S_EINVAL;
-	e->prm.freqMultiplier = multiplier;
-	if (tonality > 0) e->prm.freqTonalityLimit = tonality / std::sqrt(multiplier);
-	else e->prm.freqTonalityLimit = 1;
-	e->prm.mapN = 0;
+	for (StreamParams &p : e->hSprm) set_transpose(p, multiplier, tonality);
+	params_changed(e);
 	return 0;
 }
-int b200s_set_transpose_semitones(b200s_engine *e, float semitones, float tonality) { // :116-118
-	return b200s_set_transpose_factor(e, std::pow(2, semitones / 12), tonality);
+int b200s_set_transpose_semitones(b200s_engine *e, float semitones, float tonality) {
+	return b200s_set_transpose_factor(e, semitones_factor(semitones), tonality);
 }
-int b200s_set_formant_factor(b200s_engine *e, float multiplier, int comp) { // :124-128
+int b200s_set_formant_factor(b200s_engine *e, float multiplier, int comp) {
 	if (!e) return B200S_EINVAL;
-	e->prm.formantMultiplier = multiplier;
-	e->prm.invFormantMultiplier = 1 / multiplier;
-	e->prm.formantCompensation = comp ? 1 : 0;
+	for (StreamParams &p : e->hSprm) set_formant(p, multiplier, comp);
+	params_changed(e);
 	return 0;
 }
-int b200s_set_formant_semitones(b200s_engine *e, float semitones, int comp) { // :129-131
-	return b200s_set_formant_factor(e, std::pow(2, semitones / 12), comp);
+int b200s_set_formant_semitones(b200s_engine *e, float semitones, int comp) {
+	return b200s_set_formant_factor(e, semitones_factor(semitones), comp);
 }
 int b200s_set_formant_base(b200s_engine *e, float f) { // :133-135
 	if (!e) return B200S_EINVAL;
-	e->prm.formantBaseFreq = f;
+	for (StreamParams &p : e->hSprm) p.formantBaseFreq = f;
+	params_changed(e);
+	return 0;
+}
+int b200s_set_transpose_factor_per_stream(b200s_engine *e, const float *multipliers, const float *tonality) {
+	if (!e || !multipliers) return B200S_EINVAL;
+	for (int s = 0; s < e->S; ++s) set_transpose(e->hSprm[s], multipliers[s], tonality ? tonality[s] : 0.f);
+	params_changed(e);
+	return 0;
+}
+int b200s_set_transpose_semitones_per_stream(b200s_engine *e, const float *semitones, const float *tonality) {
+	if (!e || !semitones) return B200S_EINVAL;
+	for (int s = 0; s < e->S; ++s) set_transpose(e->hSprm[s], semitones_factor(semitones[s]), tonality ? tonality[s] : 0.f);
+	params_changed(e);
+	return 0;
+}
+int b200s_set_formant_factor_per_stream(b200s_engine *e, const float *multipliers, const int *comp) {
+	if (!e || !multipliers) return B200S_EINVAL;
+	for (int s = 0; s < e->S; ++s) set_formant(e->hSprm[s], multipliers[s], comp ? comp[s] : 0);
+	params_changed(e);
+	return 0;
+}
+int b200s_set_formant_semitones_per_stream(b200s_engine *e, const float *semitones, const int *comp) {
+	if (!e || !semitones) return B200S_EINVAL;
+	for (int s = 0; s < e->S; ++s) set_formant(e->hSprm[s], semitones_factor(semitones[s]), comp ? comp[s] : 0);
+	params_changed(e);
+	return 0;
+}
+int b200s_set_formant_base_per_stream(b200s_engine *e, const float *base) {
+	if (!e || !base) return B200S_EINVAL;
+	for (int s = 0; s < e->S; ++s) e->hSprm[s].formantBaseFreq = base[s];
+	params_changed(e);
 	return 0;
 }
 int b200s_set_freq_map_table(b200s_engine *e, const float *fin, const float *fout, int n) {
@@ -1273,14 +1409,17 @@ int b200s_set_freq_map_table(b200s_engine *e, const float *fin, const float *fou
 	CK(cudaStreamSynchronize(e->stream));
 	dfree(e->dMapIn);
 	dfree(e->dMapOut);
-	e->prm.mapN = 0;
+	e->fmap.mapN = 0;
+	for (StreamParams &p : e->hSprm) p.customMap = 1; // one table per engine, used by every stream until a transpose setter
+	params_changed(e);
 	if (n == 0) return 0;
 	int rc;
 	if ((rc = dalloc(e, &e->dMapIn, n))) return rc;
 	if ((rc = dalloc(e, &e->dMapOut, n))) return rc;
 	CK(cudaMemcpy(e->dMapIn, fin, sizeof(float) * n, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(e->dMapOut, fout, sizeof(float) * n, cudaMemcpyHostToDevice));
-	e->prm.mapN = n;
+	e->fmap.mapN = n;
+	params_changed(e);
 	return 0;
 }
 

@@ -39,8 +39,11 @@ __device__ __forceinline__ void st_stream(float *p, float v) { __stcs(p, v); }
 // the kernel's time goes with: 1 the spectrum store, 2 the window / pre-twiddle table loads (a constant instead),
 // 3 the wait for the staged input (moved to just before the next copies are issued), 4 the FFT's stages B and C.
 // ---------------------------------------------------------------------------------------------
-template <int KT, int PROBE = 0>
-__global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
+// MIXED (k_analyse2_mixed): a stereo call whose streams take both paths -- the store form is chosen per item, planar
+// rows for the streams on the mapped path (spec_il).  Otherwise (k_analyse2) the form is the call's, x.specIl, and the
+// per-item test is not in the code at all.
+template <int KT, int PROBE, bool MIXED>
+__device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	using G = PairGeo<KT>;
 	static_assert(2 * KT * sizeof(float2) <= G::LEN * sizeof(float4), "the spectrum rows of a pair fit the FFT buffer");
 	const Cfg &g = x.cfg;
@@ -157,15 +160,16 @@ __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 			const int shA = x.inAligned ? (cur.a.start & 3) : 0, shB = x.inAligned ? (cur.b.start & 3) : 0;
 			if (tid == 0) {
 				float *xw = (float *)buf;
+				const bool il = MIXED ? spec_il(x, x.call[cur.s]) : x.specIl != 0;
 				// interleaved mode: transform into scratch rows (the Y rows of block 0: the chain writes them only later), then interleave
-				float2 *tA = x.specIl ? x.Y + coef_off(x, cur.s, 0, 0) : dstA, *tB = x.specIl ? tA + KT : dstB;
+				float2 *tA = il ? x.Y + coef_off(x, cur.s, 0, 0) : dstA, *tB = il ? tA + KT : dstB;
 				for (int i = 0; i < B; ++i) xw[i] = fmul(stA[i + shA], x.window[i]);
 				emu_exact_forward(xw, B, o, 2 * KT, tA);
 				if (cur.hasB) {
 					for (int i = 0; i < B; ++i) xw[i] = fmul(stB[i + shB], x.window[i]);
 					emu_exact_forward(xw, B, o, 2 * KT, tB);
 				}
-				if (x.specIl) {
+				if (il) {
 					float4 *d4 = (float4 *)x.spec + ((size_t)cur.s * 2 * x.maxFrames + (cur.a.row >> 1)) * g.K;
 					for (int b = 0; b < KT; ++b) d4[b] = make_float4(tA[b].x, tB[b].x, tA[b].y, tB[b].y);
 				}
@@ -233,7 +237,8 @@ __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 			// defined on the idle threads too: ptxas would otherwise keep all 64 registers live around the whole loop
 			static_for<16>([&](auto qc) { v[decltype(qc)::value] = c2{f2_make(0.f, 0.f), f2_make(0.f, 0.f)}; });
 		}
-		const bool hasB = cur.hasB, il = x.specIl;
+		// (MIXED: per item, the streams on the mapped path keep planar rows; the job pairing is the same in both forms)
+		const bool hasB = cur.hasB, il = MIXED ? spec_il(x, x.call[cur.s]) : x.specIl != 0;
 		if constexpr (PROBE == 1) {
 #ifndef B200S_EMU
 			if (tid < G::M1) static_for<16>([&](auto qc) {
@@ -285,6 +290,10 @@ __global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) {
 	}
 	if (tid == 0) bulk_wait_read(); // the shared memory of the last pair's rows stays allocated until they are read
 }
+template <int KT, int PROBE = 0>
+__global__ void __launch_bounds__(256, 2) k_analyse2(Ctx x) { analyse2_body<KT, PROBE, false>(x); }
+template <int KT>
+__global__ void __launch_bounds__(256, 2) k_analyse2_mixed(Ctx x) { analyse2_body<KT, 0, true>(x); }
 
 // ---------------------------------------------------------------------------------------------
 // k_synth2: grid (C, S), 256 threads, one CTA per stream-channel; blocks of the call two at a time.

@@ -4,7 +4,9 @@ buffer-playback mode) as a batched server loop over the GPU C ABI (SURVEY.md sec
 One `LiveBatch` drives S independent streams of one `BatchStretch` engine.  Every stream has what one worklet has:
   * audio appended with `add_buffers` (web-wrapper.js:163-169) and dropped with `drop_buffers` (:137-162);
   * a TIME MAP: a list of segments {output, input, rate, active, loopStart, loopEnd} edited with `schedule` / `start` /
-    `stop` (:45-108, including `adjustPrevious`), looked up per audio quantum (:227-231);
+    `stop` (:45-108, including `adjustPrevious`), looked up per audio quantum (:227-231).  A segment may also carry the
+    worklet's parameter fields {semitones, tonalityHz, formantSemitones, formantCompensation, formantBaseHz} (defaults
+    0, 8000, 0, False, 0: :23-27); they are inherited by later points like the other fields;
   * per quantum, the segment's input position at the quantum's output time (+ latencies, loop wrap :271-279), the
     `bufferLength = inputLatency + outputLatency` samples that END there taken from the audio with zero padding on both
     sides (:282-311), and then -- exactly like the worklet, which "constantly seeks" (:313) -- `seek(window, rate)`
@@ -19,7 +21,12 @@ and its own rate.  Two ways to hand over the windows:
 When no stream is active the quantum is `process(zeros, n)` for the batch, as :247-253.  Difference from S separate
 worklets, by construction of a batch call: in a quantum where SOME streams are active, a stopped stream is fed a silent
 seek window instead of `n` zero samples appended to its history (its tail is then the synthesis ring's, up to one block
-shorter).  Parameters (transpose / formants) are batch-wide, as in the C ABI.
+shorter).
+Parameters: once some segment has carried a parameter field, every quantum hands the current segment's values of every
+stream to the engine's per-stream setters, as the worklet does (:233-235: transpose semitones with tonalityHz / sampleRate,
+formant semitones and compensation, formantBaseHz / sampleRate) -- only in quanta where some stream's values changed,
+since the engine keeps them.  A LiveBatch whose time maps never carry a parameter field never calls a setter: the
+parameters set on the engine directly stay in force.
 """
 import numpy as np
 
@@ -28,6 +35,10 @@ __all__ = ["LiveBatch"]
 
 def _segment():
     return dict(active=False, input=0.0, output=0.0, rate=1.0, loopStart=0.0, loopEnd=0.0)  # :17-29
+
+
+# the worklet's per-segment parameters and their defaults (web-wrapper.js:23-27)
+PARAM_FIELDS = dict(semitones=0.0, tonalityHz=8000.0, formantSemitones=0.0, formantCompensation=False, formantBaseHz=0.0)
 
 
 class LiveBatch:
@@ -63,6 +74,10 @@ class LiveBatch:
         self._in, self._out, self._rate, self._ls, self._le = z.copy(), z.copy(), z + 1.0, z.copy(), z.copy()
         self._active = np.zeros(self.S, bool)
         self._next = np.full(self.S, np.inf)  # output time at which the next segment takes over
+        # the current segment's parameters (one array per field) and those last handed to the engine
+        self._prm = {k: np.full(self.S, v, np.float64) for k, v in PARAM_FIELDS.items()}
+        self._prm_on = False  # some segment has carried a parameter field
+        self._prm_sent = None
 
     @property
     def current_time(self):
@@ -129,10 +144,15 @@ class LiveBatch:
         self._in[s], self._out[s], self._rate[s] = seg["input"], seg["output"], seg["rate"]
         self._ls[s], self._le[s], self._active[s] = seg["loopStart"], seg["loopEnd"], seg["active"]
         self._next[s] = tm[1]["output"] if len(tm) > 1 else np.inf
+        for k, v in PARAM_FIELDS.items():
+            if k in seg:
+                self._prm_on = True
+            self._prm[k][s] = seg.get(k, v)
 
     def schedule(self, s, obj_in, adjust_previous=False):
         """Insert a time-map point for stream `s` (semantics of the worklet's `schedule`, web-wrapper.js:67-108).
-        `obj_in`: any of outputTime (default: now), input, rate, active, loopStart, loopEnd.  Points at or after the new
+        `obj_in`: any of outputTime (default: now), input, rate, active, loopStart, loopEnd and the parameter fields
+        (PARAM_FIELDS).  Points at or after the new
         one are discarded; fields that are not given are inherited from the earliest discarded point (else from the last
         point of the map); a missing `input` is that point's playback extrapolated to the new time (or stands still if it
         was stopped).  adjust_previous: re-aim the preceding
@@ -168,8 +188,10 @@ class LiveBatch:
         self._from_map(s)
         return fresh
 
-    def start(self, s, when=None, offset=0.0, duration=None, rate=1.0):  # :49-66
+    def start(self, s, when=None, offset=0.0, duration=None, rate=1.0, semitones=None):  # :49-66
         obj = dict(active=True, input=offset, output=self.current_time + self.out_lat_s if when is None else when, rate=rate)
+        if semitones is not None:  # :57
+            obj["semitones"] = semitones
         res = self.schedule(s, obj)
         if duration is not None:
             self.stop(s, obj["output"] + duration)
@@ -177,6 +199,16 @@ class LiveBatch:
 
     def stop(self, s, when=None):  # :45-48
         return self.schedule(s, dict(active=False, output=self.current_time if when is None else when))
+
+    def _send_parameters(self):  # :233-235, for every stream at once
+        p = self._prm
+        cur = tuple(p[k].copy() for k in PARAM_FIELDS)
+        if self._prm_sent is not None and all(np.array_equal(a, b) for a, b in zip(cur, self._prm_sent)):
+            return
+        self.eng.setTransposeSemitones(p["semitones"], p["tonalityHz"] / self.sr)
+        self.eng.setFormantSemitones(p["formantSemitones"], p["formantCompensation"].astype(bool))
+        self.eng.setFormantBase(p["formantBaseHz"] / self.sr)
+        self._prm_sent = cur
 
     # ---- one audio quantum for every stream (:215-332) ----
     def process(self, n_out=128):
@@ -187,6 +219,8 @@ class LiveBatch:
             while len(tm) > 1 and tm[1]["output"] <= output_time:
                 tm.pop(0)
             self._from_map(s)
+        if self._prm_on:
+            self._send_parameters()
         if not self._active.any():  # :247-253 for the whole batch
             y = self.eng.process(np.zeros((self.S, self.C, n_out), np.float32), n_out)
         else:
