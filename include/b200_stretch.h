@@ -1,7 +1,8 @@
 /* b200_stretch.h -- C ABI of the GPU-native (H100) batched Signalsmith-Stretch hot path.
  *
  * One handle = one batch of `batch` independent audio streams that share one configuration
- * and are driven in lock-step (same call sequence, same buffer sizes), all resident on ONE GPU.
+ * and are driven in lock-step (same call sequence), all resident on ONE GPU.  Each stream has its own parameters
+ * (b200s_set_*_per_stream) and, through b200s_process_per_stream*, its own input and output length per call.
  * A batch of 1 is exactly one `signalsmith::stretch::SignalsmithStretch<float>` object.
  *
  * Every entry point mirrors one method of the reference class
@@ -140,6 +141,25 @@ int b200s_exact(b200s_engine *e, const float *in, int input_samples, float *out,
 int b200s_seek_device(b200s_engine *e, const float *d_in, int input_samples, double playback_rate);
 int b200s_process_device(b200s_engine *e, const float *d_in, int input_samples, float *d_out, int output_samples);
 int b200s_flush_device(b200s_engine *e, float *d_out, int output_samples, float playback_rate);
+/* process() with every stream's own input and output length: a server whose users each pick a tempo, whose slots idle or
+ * whose next chunks differ in length runs them in one call.  Buffers are planar [batch][channels][stride]; stream s reads
+ * the first input_samples[s] samples of each of its channel rows and writes the first output_samples[s], and the rest of
+ * each output row, up to out_stride, is written as zero.  input_samples / output_samples are host arrays of `batch` ints,
+ * copied during the call (an asynchronous caller may reuse them once the call returns).  Stream s is bit-identical to a
+ * one-stream engine with its parameters that calls process(in_s, input_samples[s], out_s, output_samples[s]) -- (0, n),
+ * (n, 0) and (0, 0) included: like the reference's process(), a (0, 0) call counts as silence.  NULL arrays, negative
+ * strides or a length outside [0, stride] return B200S_EINVAL before anything is enqueued, and b200s_last_error() names
+ * the stream.  b200s_reserve(in_stride, out_stride) sizes these calls as b200s_reserve(n_in, n_out) sizes b200s_process.
+ *   b200s_process_per_stream:         host buffers, synchronous, like b200s_process
+ *   b200s_process_per_stream_async:   host buffers, like b200s_process_async (consecutive calls whose STRIDES match pipeline
+ *                                     without a join, whatever their lengths)
+ *   b200s_process_per_stream_device:  device buffers, asynchronous on the handle's stream, like b200s_process_device */
+int b200s_process_per_stream(b200s_engine *e, const float *in, int in_stride, const int *input_samples,
+                             float *out, int out_stride, const int *output_samples);
+int b200s_process_per_stream_async(b200s_engine *e, const float *in, int in_stride, const int *input_samples,
+                                   float *out, int out_stride, const int *output_samples);
+int b200s_process_per_stream_device(b200s_engine *e, const float *d_in, int in_stride, const int *input_samples,
+                                    float *d_out, int out_stride, const int *output_samples);
 
 /* ---- measurement helpers (no reference equivalent; used by bench.py) ---- */
 /* CUDA events recorded on the handle's stream around whatever is enqueued in between. */

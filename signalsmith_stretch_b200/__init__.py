@@ -32,6 +32,7 @@ ABI_SYMBOLS = [
     "b200s_set_formant_semitones_per_stream", "b200s_set_formant_base_per_stream",
     "b200s_seek", "b200s_seek_rates", "b200s_live_seek", "b200s_output_seek", "b200s_process", "b200s_process_async", "b200s_process_pcm16", "b200s_flush", "b200s_exact",
     "b200s_seek_device", "b200s_process_device", "b200s_flush_device",
+    "b200s_process_per_stream", "b200s_process_per_stream_async", "b200s_process_per_stream_device",
     "b200s_timer_start", "b200s_timer_stop", "b200s_kernel_launches", "b200s_device_allocations", "b200s_unserved_random_blocks", "b200s_profile_begin", "b200s_profile_end",
     "b200s_selftest_divsqrt",
     "b200s_state_size", "b200s_get_state", "b200s_set_state",
@@ -98,6 +99,8 @@ def _bind(lib):
         "b200s_exact": (ci, [vp, vp, ci, vp, ci, ip]),
         "b200s_seek_device": (ci, [vp, vp, ci, cd]), "b200s_process_device": (ci, [vp, vp, ci, vp, ci]),
         "b200s_flush_device": (ci, [vp, vp, ci, cf]),
+        "b200s_process_per_stream": (ci, [vp, vp, ci, ip, vp, ci, ip]), "b200s_process_per_stream_async": (ci, [vp, vp, ci, ip, vp, ci, ip]),
+        "b200s_process_per_stream_device": (ci, [vp, vp, ci, ip, vp, ci, ip]),
         "b200s_timer_start": (ci, [vp]), "b200s_timer_stop": (ci, [vp, fp]), "b200s_kernel_launches": (cll, [vp]), "b200s_device_allocations": (cll, [vp]), "b200s_unserved_random_blocks": (cll, [vp]),
         "b200s_profile_begin": (ci, [vp]), "b200s_profile_end": (ci, [vp, fp, ip, ci]),
         "b200s_selftest_divsqrt": (ci, [vp, cll, cll, ctypes.POINTER(cll), ctypes.POINTER(cll)]),
@@ -325,8 +328,26 @@ class BatchStretch:
         x = _host(x, self._shape(n))
         self._ck(self._lib.b200s_output_seek(self._h, x.ctypes.data, n))
 
-    def process(self, inputs, outputSamples, out=None):
-        """inputs: [batch][channels][inputSamples] (numpy -> host API; torch CUDA tensor -> device API)."""
+    def _lengths(self, v, name):
+        """One sample count per stream as a contiguous int32 array (a scalar is repeated)."""
+        a = np.asarray(v)
+        if a.ndim == 0:
+            a = np.full(self.batch, int(a))
+        if a.shape != (self.batch,):
+            raise ValueError("%s: expected a scalar or %d values (one per stream), got shape %s" % (name, self.batch, np.shape(v)))
+        if not np.issubdtype(a.dtype, np.integer):
+            raise ValueError("%s: expected integer sample counts, got %s" % (name, a.dtype))
+        return np.ascontiguousarray(a, np.int32)
+
+    def process(self, inputs, outputSamples, out=None, inputSamples=None):
+        """inputs: [batch][channels][inputSamples] (numpy -> host API; torch CUDA tensor -> device API).
+
+        outputSamples: an int, or one per stream; inputSamples: None (every stream reads all of `inputs`' last dimension)
+        or one per stream.  With any per-stream array, stream s reads the first inputSamples[s] samples of its rows and
+        writes the first outputSamples[s] of an output of max(outputSamples) samples per row, zeros after them
+        (b200s_process_per_stream)."""
+        if np.ndim(outputSamples) > 0 or inputSamples is not None:
+            return self._process_per_stream(inputs, outputSamples, out, inputSamples)
         if _is_torch_cuda(inputs):
             import torch
 
@@ -344,6 +365,52 @@ class BatchStretch:
             out = np.empty(self._shape(max(outputSamples, 0)), np.float32)
         self._ck(self._lib.b200s_process(self._h, x.ctypes.data, n_in, out.ctypes.data, outputSamples))
         return out
+
+    def _process_per_stream(self, inputs, outputSamples, out, inputSamples):
+        torch_in = _is_torch_cuda(inputs)
+        n_out = self._lengths(outputSamples, "outputSamples")
+        in_stride = int(inputs.shape[-1]) if torch_in else int(np.shape(inputs)[-1])
+        n_in = self._lengths(in_stride if inputSamples is None else inputSamples, "inputSamples")
+        out_stride = int(n_out.max()) if self.batch else 0
+        if out is not None:
+            out_stride = int(out.shape[-1])
+            if tuple(out.shape) != self._shape(out_stride):
+                raise ValueError("out: expected shape %s, got %s" % (self._shape(out_stride), tuple(out.shape)))
+        for name, a, stride in (("inputSamples", n_in, in_stride), ("outputSamples", n_out, out_stride)):
+            bad = np.flatnonzero((a < 0) | (a > stride))
+            if bad.size:
+                raise ValueError("%s[%d] = %d is outside [0, %d]" % (name, bad[0], a[bad[0]], stride))
+        ip = ctypes.POINTER(ctypes.c_int)
+        if torch_in:
+            import torch
+
+            self._adopt_torch_stream()
+            assert inputs.is_contiguous() and inputs.dtype == torch.float32
+            if tuple(inputs.shape) != self._shape(in_stride):
+                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), tuple(inputs.shape)))
+            if out is None:
+                out = torch.empty(self._shape(out_stride), dtype=torch.float32, device=inputs.device)
+            self._ck(self._lib.b200s_process_per_stream_device(self._h, inputs.data_ptr(), in_stride, n_in.ctypes.data_as(ip),
+                                                               out.data_ptr(), out_stride, n_out.ctypes.data_as(ip)))
+            return out
+        x = np.asarray(inputs, np.float32)
+        if x.shape != self._shape(in_stride):
+            raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), x.shape))
+        x = _host(x, self._shape(in_stride))
+        if out is None:
+            out = np.empty(self._shape(out_stride), np.float32)
+        self._ck(self._lib.b200s_process_per_stream(self._h, x.ctypes.data, in_stride, n_in.ctypes.data_as(ip),
+                                                    out.ctypes.data, out_stride, n_out.ctypes.data_as(ip)))
+        return out
+
+    def process_per_stream_host_ptr(self, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, wait=False):
+        """Raw host pointers (pinned buffers [batch][channels][stride]) with per-stream counts n_in / n_out (`batch` ints
+        each): b200s_process_per_stream, or b200s_process_per_stream_async unless `wait` (the buffers then belong to the
+        engine until synchronize(); the counts are copied during the call)."""
+        ip = ctypes.POINTER(ctypes.c_int)
+        a, b = self._lengths(n_in, "n_in"), self._lengths(n_out, "n_out")
+        fn = self._lib.b200s_process_per_stream if wait else self._lib.b200s_process_per_stream_async
+        self._ck(fn(self._h, in_ptr, int(in_stride), a.ctypes.data_as(ip), out_ptr, int(out_stride), b.ctypes.data_as(ip)))
 
     def process_host_ptr(self, in_ptr, n_in, out_ptr, n_out):
         """Raw host pointers (e.g. pinned torch tensors): the end-to-end call bench.py times."""

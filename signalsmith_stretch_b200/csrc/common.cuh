@@ -112,6 +112,12 @@ struct Call {
 	int hasRandom;          // some block of the call stretches beyond 2x (:639): the stream takes the k_prep + k_chain path
 	int mapped;             // the stream's parameters need a frequency map or formants: mapped-path kernels, planar spectra
 	int autoPitch;          // formants with the automatic pitch estimate (formant base <= 0): k_pitch takes the stream
+	int nIn, nOut;          // the stream's input / output samples of this call (Ctx::lens, or the call's uniform counts)
+};
+
+// one stream's sample counts of a per-stream process() call (b200s_process_per_stream)
+struct CallLen {
+	int nIn, nOut;
 };
 
 // one windowed analysis FFT of the call (:333-376): block samples start at stream index `start`
@@ -176,10 +182,14 @@ struct Ctx {
 	// sub-batch of streams this launch covers (the batch is processed as a few sub-batches on
 	// prioritised CUDA streams so that different kernels of the sequence overlap on the SMs)
 	int sBase, sCount;
-	// I/O of the current call
+	// I/O of the current call.  nIn / nOut are the uniform counts; with `lens` ([S] {nIn, nOut}, b200s_process_per_stream)
+	// every stream has its own.  Only k_plan reads either: it resolves them into Call::nIn / nOut, which every later kernel
+	// of the call reads.  outTail > 0 (per-stream calls): output samples from Call::nOut up to outTail are written as zero.
 	const float *in;
 	float *out;
 	int nIn, nOut;
+	const CallLen *lens;
+	int outTail;
 	long long inStreamStride, outStreamStride; // floats between streams
 	int inChanStride, outChanStride;           // floats between channels
 };

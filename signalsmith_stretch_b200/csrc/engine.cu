@@ -65,7 +65,14 @@ struct b200s_engine {
 	cudaStream_t subStream[kMaxSub] = {};
 	cudaEvent_t evBegin = 0, evSubDone[kMaxSub] = {};
 	int chainedGroups = 0; // > 0: the last operation was a host-buffer process() over this many stream groups (see process_impl)
-	int chainedIn = -1, chainedOut = -1; // its per-channel sample counts: the groups' slabs of the staging buffers sit at sBase*C*n
+	int chainedIn = -1, chainedOut = -1; // its per-channel sample counts (strides): the groups' slabs of the staging buffers sit at sBase*C*n
+	// per-stream sample counts (b200s_process_per_stream): the device table Ctx::lens [S], allocated at configure, and two
+	// pinned staging copies.  Each stream group copies its own slice on its own CUDA stream ahead of its k_plan, so chained
+	// calls need no join for it; a staging copy is rewritten once every group's copy issued from it two calls ago has run.
+	CallLen *dLens = 0;
+	CallLen *pinLens[2] = {0, 0};
+	cudaEvent_t evLens[2][kMaxSub] = {};
+	int lensSlot = 0;
 	int chainV = 0, fftV1 = 0; // b200s_set_tuning overrides (0 = default)
 	int exactMath = 0;         // b200s_set_tuning key 3: 1 = the phase chain in the reference's unfused IEEE arithmetic
 	// host-buffer API: stream groups whose H2D copy / kernels / D2H copy are pipelined.  H100 SXM, batch 1024 stereo, one run
@@ -652,6 +659,7 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 		if ((rc = dalloc(e, &e->dSprm, (size_t)g.S))) return rc;
 		e->sprmDirty = true;
 	}
+	if (!e->dLens && (rc = dalloc(e, &e->dLens, (size_t)g.S))) return rc; // per-stream sample counts (filled by every per-stream call)
 
 	// ---- state
 	const size_t SC = (size_t)g.S * g.C;
@@ -820,16 +828,35 @@ static int ensure_buf(b200s_engine *e, float **p, size_t *cap, size_t n, bool ze
 // hIn / hOut (host-buffer API only): packed [S][C][n] host arrays mirrored by dIn / dOut; each stream group
 // then copies its own slab in, runs its kernels and copies its slab out on its own CUDA stream, so that the
 // PCIe transfers of one group overlap the kernels of the others.
+// lenIn / lenOut (b200s_process_per_stream, validated by the caller): host arrays of S per-stream sample counts; nIn / nOut
+// are then the rows' strides, stream s reads lenIn[s] samples of each row and writes lenOut[s], zeros up to the stride.
+// Without them every stream reads nIn and writes nOut.
 static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, long long inStreamStride, int nIn,
                         float *dOut, int outChanStride, long long outStreamStride, int nOut,
-                        const float *hIn = nullptr, float *hOut = nullptr, const short *hIn16 = nullptr, short *hOut16 = nullptr) {
+                        const float *hIn = nullptr, float *hOut = nullptr, const short *hIn16 = nullptr, short *hOut16 = nullptr,
+                        const int *lenIn = nullptr, const int *lenOut = nullptr) {
 	const Cfg &g = e->cfg;
 	if (nIn < 0 || nOut < 0) {
 		e->err = "process: negative sample count";
 		return B200S_EINVAL;
 	}
+	const bool perStream = lenIn && lenOut;
+	// the host's decisions over the streams' counts: the longest output sizes the scratch and the grids; a call may need the
+	// random path when ANY stream may stretch beyond 2x; bulk-copy staging needs every input length a multiple of 4
+	int maxOut = nOut;
+	bool lowRatio = nOut > 0 && (long long)nIn * 2 * g.H < (long long)nOut * (g.H + 4), anyIdle = false, lensAligned = nIn % 4 == 0;
+	if (perStream) {
+		maxOut = 0;
+		lowRatio = false;
+		for (int s = 0; s < g.S; ++s) {
+			maxOut = std::max(maxOut, lenOut[s]);
+			if (lenOut[s] > 0) lowRatio = lowRatio || (long long)lenIn[s] * 2 * g.H < (long long)lenOut[s] * (g.H + 4);
+			else anyIdle = true;
+			lensAligned = lensAligned && lenIn[s] % 4 == 0;
+		}
+	}
 	int rc;
-	if ((rc = ensure_scratch(e, nOut))) return rc;
+	if ((rc = ensure_scratch(e, maxOut))) return rc;
 	if (e->sprmDirty) {
 		// new per-stream parameters, on the main stream ahead of this call's work.  This call then joins (see `chained`
 		// below): a chained call's stream groups do not wait for the main stream, so they could read the new table while
@@ -846,11 +873,12 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	// input interval is interval * nIn / nOut give or take a sample; the first block's mixes in the previous call's ratio;
 	// after a seek it is 1 / playbackRate.  Conservative on purpose: the decision itself is taken per stream on the device
 	// (k_plan sets Call::hasRandom); this only says whether the kernels of the random path have to be launched at all.
-	const bool lowRatio = nOut > 0 && (long long)nIn * 2 * g.H < (long long)nOut * (g.H + 4);
-	const bool mayRandom = nOut > 0 && (lowRatio || e->prevCallMayRandom || e->seekMayRandom);
-	if (nOut > 0) {
-		e->prevCallMayRandom = lowRatio;
-		e->seekMayRandom = false;
+	// (Per stream: a stream that produces no output keeps its previous ratio or its seek's time factor for its next block,
+	// so while one does, the flags carry over.)
+	const bool mayRandom = maxOut > 0 && (lowRatio || e->prevCallMayRandom || e->seekMayRandom);
+	if (maxOut > 0) {
+		e->prevCallMayRandom = lowRatio || (anyIdle && e->prevCallMayRandom);
+		e->seekMayRandom = anyIdle && e->seekMayRandom;
 	}
 	// Each stream takes the path its own parameters need (k_plan sets Call::mapped); a call launches the kernels of the paths
 	// some stream takes, and every kernel skips the streams of the other path.  With the same parameters on every stream
@@ -866,8 +894,16 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	x.in = dIn; x.out = dOut; x.nIn = nIn; x.nOut = nOut;
 	x.inChanStride = inChanStride; x.inStreamStride = inStreamStride;
 	x.outChanStride = outChanStride; x.outStreamStride = outStreamStride;
-	x.inAligned = ((uintptr_t)dIn % 16 == 0) && inChanStride % 4 == 0 && inStreamStride % 4 == 0 && nIn % 4 == 0 && g.histLen % 4 == 0;
-	const int F = frames_bound(g, nOut);
+	x.inAligned = ((uintptr_t)dIn % 16 == 0) && inChanStride % 4 == 0 && inStreamStride % 4 == 0 && lensAligned && g.histLen % 4 == 0;
+	const int F = frames_bound(g, maxOut);
+	int lk = 0;
+	if (perStream) { // this call's counts into a staging copy; the stream groups upload their slices below
+		lk = e->lensSlot ^= 1;
+		for (int i = 0; i < b200s_engine::kMaxSub; ++i) CK(cudaEventSynchronize(e->evLens[lk][i]));
+		for (int s = 0; s < g.S; ++s) e->pinLens[lk][s] = CallLen{lenIn[s], lenOut[s]};
+		x.lens = e->dLens;
+		x.outTail = nOut;
+	}
 	// Sub-batch pipeline: the streams of the batch are independent, so the launch sequence is issued
 	// per sub-batch on its own CUDA stream (descending priority).  Sub-batch 0's chain then runs while
 	// sub-batch 1 is still in its FFT kernel, and so on: the latency-bound wavefront kernel and the
@@ -882,7 +918,8 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	// call n+1 may start its H2D copy while other groups still finish call n (b200s_process_async pipelines calls this
 	// way).  Anything else first joins: the main stream has waited for every group at the end of the previous call.
 	// The groups' slabs of the shared staging buffers sit at sBase*C*nIn / sBase*C*nOut, so they only coincide from call to
-	// call when the sample counts do: a call with different counts must first join (otherwise group g's copy of call n+1
+	// call when the sample counts (the strides of a per-stream call; its streams' own counts may differ) do: a call with
+	// different counts must first join (otherwise group g's copy of call n+1
 	// could overwrite the slab a neighbouring group still uses for call n); evBegin below is that join, since the main
 	// stream has waited for every group's evSubDone at the end of the previous call.
 	const bool chained = hostIO && nSub > 1 && e->chainedGroups == nSub && e->chainedIn == nIn && e->chainedOut == nOut;
@@ -898,6 +935,10 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 		if (nSub > 1 && !chained) CK(cudaStreamWaitEvent(st, e->evBegin, 0));
 		x.sBase = (int)((long long)g.S * sub / nSub);
 		x.sCount = (int)((long long)g.S * (sub + 1) / nSub) - x.sBase;
+		if (perStream) { // the group's slice of the counts, ordered before its k_plan and after its previous call's kernels
+			CK(cudaMemcpyAsync(e->dLens + x.sBase, e->pinLens[lk] + x.sBase, sizeof(CallLen) * x.sCount, cudaMemcpyHostToDevice, st));
+			CK(cudaEventRecord(e->evLens[lk][sub], st));
+		}
 		if (hIn && nIn > 0)
 			CK(cudaMemcpyAsync((float *)dIn + (size_t)x.sBase * g.C * nIn, hIn + (size_t)x.sBase * g.C * nIn, sizeof(float) * (size_t)x.sCount * g.C * nIn, cudaMemcpyHostToDevice, st));
 		if (hIn16 && nIn > 0) { // 16-bit PCM: 2 bytes per sample over PCIe, converted on the device
@@ -991,7 +1032,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 				} else if (chainV >= 3) {
 					PROF(PK_CHAIN, B200S_LAUNCH(chain3_kernel(g, chainV, !e->exactMath), dim3(x.sCount), dim3(32), chainV >= 6 ? smem_chain6() : chainV == 4 ? smem_chain4(g.L) : sizeof(Chain3Tiles), st, x));
 				} else if (chainV == 2) {
-					const int W = chain2_warps(g, nOut);
+					const int W = chain2_warps(g, maxOut);
 					ChainKernel kc = chain2_kernel(g, g.C == 1 && !e->exactMath);
 					int _rc;
 					if ((_rc = prof_mark(e, PK_CHAIN, true))) return _rc;
@@ -1195,13 +1236,17 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 		    cudaEventCreateWithFlags(&e->evJoin, cudaEventDisableTiming) != cudaSuccess)
 			e->commitStream = 0; // (no fork then: the commit follows the synthesis on the main stream)
 	}
-	for (int k = 0; k < 2; ++k)
-		if (!host_alloc((void **)&e->pinSprm[k], sizeof(StreamParams) * (size_t)batch) ||
-		    cudaEventCreateWithFlags(&e->evSprm[k], cudaEventDisableTiming) != cudaSuccess) {
+	for (int k = 0; k < 2; ++k) {
+		bool ok = host_alloc((void **)&e->pinSprm[k], sizeof(StreamParams) * (size_t)batch) &&
+		          cudaEventCreateWithFlags(&e->evSprm[k], cudaEventDisableTiming) == cudaSuccess &&
+		          host_alloc((void **)&e->pinLens[k], sizeof(CallLen) * (size_t)batch);
+		for (int i = 0; i < b200s_engine::kMaxSub && ok; ++i) ok = cudaEventCreateWithFlags(&e->evLens[k][i], cudaEventDisableTiming) == cudaSuccess;
+		if (!ok) {
 			g_createError = "pinned host memory / event creation failed";
 			b200s_destroy(e);
 			return B200S_ECUDA;
 		}
+	}
 	{ // sub-batch streams: highest priority first
 		int lo = 0, hi = 0;
 		cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -1234,9 +1279,13 @@ void b200s_destroy(b200s_engine *e) {
 	dfree(e->dSeekStf);
 	dfree(e->dSeekEnd);
 	dfree(e->dSprm);
+	dfree(e->dLens);
 	for (int k = 0; k < 2; ++k) {
 		host_free(e->pinSprm[k]);
 		if (e->evSprm[k]) cudaEventDestroy(e->evSprm[k]);
+		host_free(e->pinLens[k]);
+		for (int i = 0; i < b200s_engine::kMaxSub; ++i)
+			if (e->evLens[k][i]) cudaEventDestroy(e->evLens[k][i]);
 	}
 	for (int i = 0; i < b200s_engine::kMaxSub; ++i) {
 		if (e->subStream[i]) cudaStreamDestroy(e->subStream[i]);
@@ -1504,6 +1553,57 @@ int b200s_process_async(b200s_engine *e, const float *in, int nIn, float *out, i
 	if ((rc = stage_in(e, nullptr, nIn))) return rc;
 	if ((rc = stage_out(e, nOut))) return rc;
 	return process_impl(e, e->dIn, nIn, (long long)e->cfg.C * nIn, nIn, e->dOut, nOut, (long long)e->cfg.C * nOut, nOut, in, out);
+}
+// Arguments of the per-stream process calls, checked before anything is enqueued
+static int check_per_stream(b200s_engine *e, const char *fn, int inStride, const int *nIn, int outStride, const int *nOut) {
+	if (!nIn || !nOut) {
+		e->err = std::string(fn) + ": input_samples and output_samples must not be NULL";
+		return B200S_EINVAL;
+	}
+	if (inStride < 0 || outStride < 0) {
+		e->err = std::string(fn) + ": negative stride";
+		return B200S_EINVAL;
+	}
+	for (int s = 0; s < e->S; ++s) {
+		const bool badIn = nIn[s] < 0 || nIn[s] > inStride;
+		if (badIn || nOut[s] < 0 || nOut[s] > outStride) {
+			e->err = std::string(fn) + ": stream " + std::to_string(s) + ": " + (badIn ? "input_samples " : "output_samples ") +
+			         std::to_string(badIn ? nIn[s] : nOut[s]) + " is outside [0, " + std::to_string(badIn ? inStride : outStride) + "]";
+			return B200S_EINVAL;
+		}
+	}
+	return 0;
+}
+int b200s_process_per_stream(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {
+	NEED_CFG();
+	int rc;
+	if ((rc = check_per_stream(e, "b200s_process_per_stream", inStride, nIn, outStride, nOut))) return rc;
+	if ((rc = stage_in(e, nullptr, inStride))) return rc; // capacity only: the copies are issued per stream group
+	if ((rc = stage_out(e, outStride))) return rc;
+	const long long C = e->cfg.C;
+	if ((rc = process_impl(e, e->dIn, inStride, C * inStride, inStride, e->dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, nIn, nOut))) return rc;
+	CK(cudaStreamSynchronize(e->stream));
+	return 0;
+}
+int b200s_process_per_stream_async(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {
+	NEED_CFG();
+	int rc;
+	if ((rc = check_per_stream(e, "b200s_process_per_stream_async", inStride, nIn, outStride, nOut))) return rc;
+	if ((size_t)e->cfg.S * e->cfg.C * std::max(inStride, 1) > e->inCap || (size_t)e->cfg.S * e->cfg.C * std::max(outStride, 1) > e->outCap || !e->dIn || !e->dOut) {
+		// growing the staging buffers would invalidate copies still in flight: drain first
+		CK(cudaStreamSynchronize(e->stream));
+	}
+	if ((rc = stage_in(e, nullptr, inStride))) return rc;
+	if ((rc = stage_out(e, outStride))) return rc;
+	const long long C = e->cfg.C;
+	return process_impl(e, e->dIn, inStride, C * inStride, inStride, e->dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, nIn, nOut);
+}
+int b200s_process_per_stream_device(b200s_engine *e, const float *dIn, int inStride, const int *nIn, float *dOut, int outStride, const int *nOut) {
+	NEED_CFG();
+	int rc;
+	if ((rc = check_per_stream(e, "b200s_process_per_stream_device", inStride, nIn, outStride, nOut))) return rc;
+	const long long C = e->cfg.C;
+	return process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, nullptr, nullptr, nullptr, nullptr, nIn, nOut);
 }
 int b200s_flush(b200s_engine *e, float *out, int nOut, float rate) {
 	NEED_CFG();

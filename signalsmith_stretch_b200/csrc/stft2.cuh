@@ -56,17 +56,18 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	const long long total = (long long)x.sCount * PJ;
 
 	struct Item {
-		int s, hasB;
+		int s, hasB, nIn; // nIn: the stream's Call::nIn (loaded with the descriptors, off the staging path)
 		Job a, b;
 	};
 	// item -> jobs; false when the stream has fewer pairs than slots
-	// (the three loads are independent of each other: the job slots exist even when the stream has fewer jobs)
+	// (the four loads are independent of each other: the job slots exist even when the stream has fewer jobs)
 	// fetch_raw only issues the loads (m.hasB temporarily holds the stream's job count); fetch_done turns them into
 	// an item.  Keeping the two apart lets the loads of the item after next fly for a whole iteration.
 	auto fetch_raw = [&](long long it, Item &m) {
 		m.s = x.sBase + (int)(it / PJ);
 		const Job *jb = x.jobs + (size_t)m.s * 2 * g.C * x.maxFrames + 2 * (int)(it % PJ);
 		m.hasB = x.call[m.s].nJobs;
+		m.nIn = x.call[m.s].nIn;
 		m.a = jb[0];
 		m.b = jb[1];
 	};
@@ -95,14 +96,14 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	fence_async_proxy();
 	__syncthreads();
 	unsigned stagePar = 0u;
-	auto stage_job = [&](float *st, int s, const Job &j, int t0, int nT) {
+	auto stage_job = [&](float *st, int s, int nIn, const Job &j, int t0, int nT) {
 		const float *ib = x.in + (size_t)s * x.inStreamStride + (size_t)j.c * x.inChanStride;
 		const float *he = x.histCur + ((size_t)s * g.C + j.c) * g.histLen + g.histLen;
 		if (x.inAligned) {
 			const int sh = j.start & 3, a00 = j.start - sh, nCh = (B + sh + 3) >> 2;
 			// chunk q holds samples a00 + 4q ..: [qh0, z) comes from the history, [z, qi1) from the input
 			const int z = min(max((-a00) >> 2, 0), nCh);
-			const int qh0 = min(max((-g.histLen - a00) >> 2, 0), z), qi1 = min(max((x.nIn - a00) >> 2, z), nCh);
+			const int qh0 = min(max((-g.histLen - a00) >> 2, 0), z), qi1 = min(max((nIn - a00) >> 2, z), nCh);
 			if (tid == t0) {
 				fence_async_proxy(); // the staging buffer was last read through the generic proxy
 				mbar_expect(&stageBar, 16u * (unsigned)(qi1 - qh0));
@@ -114,7 +115,7 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 		} else {
 			for (int i = tid; i < B; i += nT) {
 				const int a = j.start + i;
-				if (a < x.nIn && a >= -g.histLen) cp_async4(st + i, a >= 0 ? ib + a : he + a);
+				if (a < nIn && a >= -g.histLen) cp_async4(st + i, a >= 0 ? ib + a : he + a);
 				else st[i] = 0.f;
 			}
 		}
@@ -126,8 +127,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	Item cur, nxt;
 	long long item = next_valid(blockIdx.x, cur);
 	if (item < total) {
-		stage_job(stA, cur.s, cur.a, 0, 256);
-		stage_job(stB, cur.s, cur.b, 32, 256);
+		stage_job(stA, cur.s, cur.nIn, cur.a, 0, 256);
+		stage_job(stB, cur.s, cur.nIn, cur.b, 32, 256);
 	}
 	long long nitem = item < total ? next_valid(item + gridDim.x, nxt) : total;
 	while (item < total) {
@@ -178,8 +179,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 			item = nitem;
 			cur = nxt;
 			if (item < total) {
-				stage_job(stA, cur.s, cur.a, 0, 256);
-				stage_job(stB, cur.s, cur.b, 32, 256);
+				stage_job(stA, cur.s, cur.nIn, cur.a, 0, 256);
+				stage_job(stB, cur.s, cur.nIn, cur.b, 32, 256);
 				nitem = next_valid(item + gridDim.x, nxt);
 			}
 			continue;
@@ -215,8 +216,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 			}
 		}
 		if (nitem < total) { // start the next pair's input on its way while this FFT runs
-			stage_job(stA, nxt.s, nxt.a, 0, 256);
-			stage_job(stB, nxt.s, nxt.b, 32, 256);
+			stage_job(stA, nxt.s, nxt.nIn, nxt.a, 0, 256);
+			stage_job(stB, nxt.s, nxt.nIn, nxt.b, 32, 256);
 			if (cand < total) fetch_raw(cand, n2); // descriptor of the item after next: loads in flight until the end of the iteration
 		}
 		if constexpr (PROBE != 4) pair_dit_stage_b<KT>(buf, tw, tid);
@@ -314,7 +315,8 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 	float *out = x.out + (size_t)s * x.outStreamStride + (size_t)c * x.outChanStride;
 	if (cl.bypass) { // :252-267
 		const float *in = x.in + (size_t)s * x.inStreamStride + (size_t)c * x.inChanStride;
-		for (int i = tid; i < x.nOut; i += 256) out[i] = x.nIn > 0 ? in[i % x.nIn] : 0.f;
+		for (int i = tid; i < cl.nOut; i += 256) out[i] = cl.nIn > 0 ? in[i % cl.nIn] : 0.f;
+		for (int i = cl.nOut + tid; i < x.outTail; i += 256) out[i] = 0.f;
 		return;
 	}
 	const int P = g.pendLen, B = g.B, o = g.o, addOff = g.addOff;
@@ -495,7 +497,12 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 		}
 		__syncthreads();
 	}
-	emit(x.nOut - emitted);
+	{
+		// (re-read here: a register that holds the count through the block loop costs the kernel spills)
+		const int nOut = __ldg(&x.call[s].nOut);
+		emit(nOut - emitted);
+		for (int i = nOut + tid; i < x.outTail; i += 256) st_stream(out + i, 0.f); // (per-stream calls: the row's zero tail)
+	}
 	__syncthreads();
 	for (int i = tid; i < P; i += 256) {
 		int p = head + i;
