@@ -160,6 +160,33 @@ int b200s_process_per_stream_async(b200s_engine *e, const float *in, int in_stri
                                    float *out, int out_stride, const int *output_samples);
 int b200s_process_per_stream_device(b200s_engine *e, const float *d_in, int in_stride, const int *input_samples,
                                     float *d_out, int out_stride, const int *output_samples);
+/* One call in which every stream runs its own operation: a server turns one slot over (flush the track that ended,
+ * outputSeek into the next one) while the other slots keep processing.  ops[s] is one of B200S_OP_*; buffers and counts are
+ * those of b200s_process_per_stream, and playback_rates[s] (host array, may be NULL when no stream seeks: every FLUSH is
+ * then at rate 0, the reference's default) is the rate of a SEEK or FLUSH.  Stream s is bit-identical to a one-stream
+ * engine with its parameters that calls the reference method its op names, in the same order, and does nothing for its
+ * SKIP calls -- outputs and every piece of state.  Every output sample an op does not produce is written as zero, up to
+ * out_stride (the whole row for SEEK, OUTPUT_SEEK, RESET and SKIP).  exact() is OUTPUT_SEEK, PROCESS, FLUSH over three calls.
+ * B200S_EINVAL, before anything is enqueued and with b200s_last_error() naming the stream: NULL ops or count arrays, a
+ * negative stride, an op out of range, SEEK without rates, a count the op does not use (input for FLUSH / RESET / SKIP,
+ * output for SEEK / OUTPUT_SEEK / RESET / SKIP), a count outside [0, stride].  b200s_reserve(in_stride, out_stride) also
+ * sizes the flushes (up to in_stride zero samples) and output seeks of these calls; a FLUSH at a rate below 1/2 (rate 0,
+ * the default, included) stretches beyond 2x and, like any call beyond 2x, allocates the random path's rows on first use.
+ * A call of PROCESS / SKIP ops pipelines like b200s_process_per_stream_async; a call with any other op joins. */
+enum {
+	B200S_OP_SKIP = 0,        /* the stream sits this call out: state untouched, output row written as zero */
+	B200S_OP_PROCESS = 1,     /* process(in, input_samples[s], out, output_samples[s])          :209-423 */
+	B200S_OP_SEEK = 2,        /* seek(in, input_samples[s], playback_rates[s])                    :139-165 */
+	B200S_OP_OUTPUT_SEEK = 3, /* outputSeek(in, input_samples[s])                                 :172-204 */
+	B200S_OP_FLUSH = 4,       /* flush(out, output_samples[s], (float)playback_rates[s])          :426-464 */
+	B200S_OP_RESET = 5        /* reset()                                                          :49-60   */
+};
+int b200s_run_per_stream(b200s_engine *e, const int *ops, const float *in, int in_stride, const int *input_samples,
+                         float *out, int out_stride, const int *output_samples, const double *playback_rates);
+int b200s_run_per_stream_async(b200s_engine *e, const int *ops, const float *in, int in_stride, const int *input_samples,
+                               float *out, int out_stride, const int *output_samples, const double *playback_rates);
+int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *d_in, int in_stride, const int *input_samples,
+                                float *d_out, int out_stride, const int *output_samples, const double *playback_rates);
 
 /* ---- measurement helpers (no reference equivalent; used by bench.py) ---- */
 /* CUDA events recorded on the handle's stream around whatever is enqueued in between. */
@@ -180,7 +207,8 @@ long long b200s_device_allocations(const b200s_engine *e);
 long long b200s_unserved_random_blocks(b200s_engine *e);
 /* Per-kernel device time of process(): between begin and end every kernel of the process()
  * launch sequence is bracketed by CUDA events on the handle's stream.  `ms`/`counts` receive, in
- * this order: plan, analyse, prep, chain, synth, commit (n >= 6). */
+ * this order: plan, analyse, prep, chain, synth, commit (n >= 6), then, with n >= 7, the pre and post phases of
+ * b200s_run_per_stream (dropped when n == 6). */
 int b200s_profile_begin(b200s_engine *e);
 int b200s_profile_end(b200s_engine *e, float *ms, int *counts, int n);
 

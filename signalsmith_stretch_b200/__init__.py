@@ -33,6 +33,7 @@ ABI_SYMBOLS = [
     "b200s_seek", "b200s_seek_rates", "b200s_live_seek", "b200s_output_seek", "b200s_process", "b200s_process_async", "b200s_process_pcm16", "b200s_flush", "b200s_exact",
     "b200s_seek_device", "b200s_process_device", "b200s_flush_device",
     "b200s_process_per_stream", "b200s_process_per_stream_async", "b200s_process_per_stream_device",
+    "b200s_run_per_stream", "b200s_run_per_stream_async", "b200s_run_per_stream_device",
     "b200s_timer_start", "b200s_timer_stop", "b200s_kernel_launches", "b200s_device_allocations", "b200s_unserved_random_blocks", "b200s_profile_begin", "b200s_profile_end",
     "b200s_selftest_divsqrt",
     "b200s_state_size", "b200s_get_state", "b200s_set_state",
@@ -101,6 +102,9 @@ def _bind(lib):
         "b200s_flush_device": (ci, [vp, vp, ci, cf]),
         "b200s_process_per_stream": (ci, [vp, vp, ci, ip, vp, ci, ip]), "b200s_process_per_stream_async": (ci, [vp, vp, ci, ip, vp, ci, ip]),
         "b200s_process_per_stream_device": (ci, [vp, vp, ci, ip, vp, ci, ip]),
+        "b200s_run_per_stream": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
+        "b200s_run_per_stream_async": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
+        "b200s_run_per_stream_device": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
         "b200s_timer_start": (ci, [vp]), "b200s_timer_stop": (ci, [vp, fp]), "b200s_kernel_launches": (cll, [vp]), "b200s_device_allocations": (cll, [vp]), "b200s_unserved_random_blocks": (cll, [vp]),
         "b200s_profile_begin": (ci, [vp]), "b200s_profile_end": (ci, [vp, fp, ip, ci]),
         "b200s_selftest_divsqrt": (ci, [vp, cll, cll, ctypes.POINTER(cll), ctypes.POINTER(cll)]),
@@ -144,6 +148,8 @@ class BatchStretch:
     """A batch of independent streams; one `SignalsmithStretch<float>` per stream (signalsmith-stretch.h:34)."""
 
     version = (1, 3, 2)  # :36
+    # per-stream operations of run() (B200S_OP_* of include/b200_stretch.h)
+    OP_SKIP, OP_PROCESS, OP_SEEK, OP_OUTPUT_SEEK, OP_FLUSH, OP_RESET = range(6)
 
     def __init__(self, batch=1, seed=0, device=0, lib_path=None):
         self._lib = _load(lib_path or library_path())
@@ -367,10 +373,32 @@ class BatchStretch:
         return out
 
     def _process_per_stream(self, inputs, outputSamples, out, inputSamples):
+        return self.run(self.OP_PROCESS, inputs, outputSamples, inputSamples=inputSamples, out=out)
+
+    def run(self, ops, inputs, outputSamples, inputSamples=None, playbackRates=None, out=None):
+        """Every stream runs its own operation (b200s_run_per_stream): ops, outputSamples, inputSamples and playbackRates are
+        scalars (repeated for every stream) or one value per stream.  OP_PROCESS: process(inputs[s][:, :inputSamples[s]],
+        outputSamples[s]); OP_SEEK: seek(inputs[s][:, :inputSamples[s]], playbackRates[s]); OP_OUTPUT_SEEK:
+        outputSeek(inputs[s][:, :inputSamples[s]]); OP_FLUSH: flush(outputSamples[s], playbackRates[s]); OP_RESET: reset();
+        OP_SKIP: nothing.  inputs: [batch][channels][stride] (numpy -> host API; torch CUDA tensor -> device API; None
+        when no stream reads input); inputSamples defaults to the whole stride for the ops that read input and 0 for the
+        others.  Returns [batch][channels][max(outputSamples)] (or `out`), zeros after each stream's own output."""
         torch_in = _is_torch_cuda(inputs)
+        op = self._lengths(ops, "ops")
+        if np.any((op < 0) | (op > 5)):
+            raise ValueError("ops: every op must be one of OP_SKIP .. OP_RESET")
         n_out = self._lengths(outputSamples, "outputSamples")
-        in_stride = int(inputs.shape[-1]) if torch_in else int(np.shape(inputs)[-1])
-        n_in = self._lengths(in_stride if inputSamples is None else inputSamples, "inputSamples")
+        in_stride = 0 if inputs is None else int(inputs.shape[-1]) if torch_in else int(np.shape(inputs)[-1])
+        if inputSamples is None:
+            reads = (op == self.OP_PROCESS) | (op == self.OP_SEEK) | (op == self.OP_OUTPUT_SEEK)
+            inputSamples = np.where(reads, in_stride, 0)
+        n_in = self._lengths(inputSamples, "inputSamples")
+        rates = None
+        if playbackRates is not None:
+            rates = np.ascontiguousarray(np.broadcast_to(np.asarray(playbackRates, np.float64), (self.batch,)) if np.ndim(playbackRates) == 0
+                                         else np.asarray(playbackRates, np.float64))
+            if rates.shape != (self.batch,):
+                raise ValueError("playbackRates: expected a scalar or %d values, got shape %s" % (self.batch, np.shape(playbackRates)))
         out_stride = int(n_out.max()) if self.batch else 0
         if out is not None:
             out_stride = int(out.shape[-1])
@@ -380,7 +408,8 @@ class BatchStretch:
             bad = np.flatnonzero((a < 0) | (a > stride))
             if bad.size:
                 raise ValueError("%s[%d] = %d is outside [0, %d]" % (name, bad[0], a[bad[0]], stride))
-        ip = ctypes.POINTER(ctypes.c_int)
+        ip, dp = ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_double)
+        rp = None if rates is None else rates.ctypes.data_as(dp)
         if torch_in:
             import torch
 
@@ -390,17 +419,19 @@ class BatchStretch:
                 raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), tuple(inputs.shape)))
             if out is None:
                 out = torch.empty(self._shape(out_stride), dtype=torch.float32, device=inputs.device)
-            self._ck(self._lib.b200s_process_per_stream_device(self._h, inputs.data_ptr(), in_stride, n_in.ctypes.data_as(ip),
-                                                               out.data_ptr(), out_stride, n_out.ctypes.data_as(ip)))
+            self._ck(self._lib.b200s_run_per_stream_device(self._h, op.ctypes.data_as(ip), inputs.data_ptr(), in_stride, n_in.ctypes.data_as(ip),
+                                                           out.data_ptr(), out_stride, n_out.ctypes.data_as(ip), rp))
             return out
-        x = np.asarray(inputs, np.float32)
-        if x.shape != self._shape(in_stride):
-            raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), x.shape))
-        x = _host(x, self._shape(in_stride))
+        x = None
+        if inputs is not None:
+            x = np.asarray(inputs, np.float32)
+            if x.shape != self._shape(in_stride):
+                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), x.shape))
+            x = _host(x, self._shape(in_stride))
         if out is None:
             out = np.empty(self._shape(out_stride), np.float32)
-        self._ck(self._lib.b200s_process_per_stream(self._h, x.ctypes.data, in_stride, n_in.ctypes.data_as(ip),
-                                                    out.ctypes.data, out_stride, n_out.ctypes.data_as(ip)))
+        self._ck(self._lib.b200s_run_per_stream(self._h, op.ctypes.data_as(ip), None if x is None else x.ctypes.data, in_stride,
+                                                n_in.ctypes.data_as(ip), out.ctypes.data, out_stride, n_out.ctypes.data_as(ip), rp))
         return out
 
     def process_per_stream_host_ptr(self, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, wait=False):
@@ -411,6 +442,17 @@ class BatchStretch:
         a, b = self._lengths(n_in, "n_in"), self._lengths(n_out, "n_out")
         fn = self._lib.b200s_process_per_stream if wait else self._lib.b200s_process_per_stream_async
         self._ck(fn(self._h, in_ptr, int(in_stride), a.ctypes.data_as(ip), out_ptr, int(out_stride), b.ctypes.data_as(ip)))
+
+    def run_per_stream_host_ptr(self, ops, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, playback_rates=None, wait=False):
+        """Raw host pointers (pinned buffers [batch][channels][stride]) with per-stream ops and counts (`batch` values each):
+        b200s_run_per_stream, or b200s_run_per_stream_async unless `wait` (the buffers then belong to the engine until
+        synchronize(); ops, counts and rates are copied during the call)."""
+        ip = ctypes.POINTER(ctypes.c_int)
+        o, a, b = self._lengths(ops, "ops"), self._lengths(n_in, "n_in"), self._lengths(n_out, "n_out")
+        r = None if playback_rates is None else np.ascontiguousarray(np.broadcast_to(np.asarray(playback_rates, np.float64), (self.batch,)))
+        rp = None if r is None else r.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        fn = self._lib.b200s_run_per_stream if wait else self._lib.b200s_run_per_stream_async
+        self._ck(fn(self._h, o.ctypes.data_as(ip), in_ptr, int(in_stride), a.ctypes.data_as(ip), out_ptr, int(out_stride), b.ctypes.data_as(ip), rp))
 
     def process_host_ptr(self, in_ptr, n_in, out_ptr, n_out):
         """Raw host pointers (e.g. pinned torch tensors): the end-to-end call bench.py times."""
@@ -481,12 +523,14 @@ class BatchStretch:
     def profile_begin(self):
         self._ck(self._lib.b200s_profile_begin(self._h))
 
-    def profile_end(self):
-        """{kernel: (total ms, launches)} for the process() calls since profile_begin()."""
-        ms = (ctypes.c_float * 6)()
-        cnt = (ctypes.c_int * 6)()
-        self._ck(self._lib.b200s_profile_end(self._h, ms, cnt, 6))
-        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(self.KERNELS)}
+    def profile_end(self, phases=False):
+        """{kernel: (total ms, launches)} for the process() calls since profile_begin(); phases=True adds "phases", the pre
+        and post phases of run()."""
+        names = self.KERNELS + (("phases",) if phases else ())
+        ms = (ctypes.c_float * len(names))()
+        cnt = (ctypes.c_int * len(names))()
+        self._ck(self._lib.b200s_profile_end(self._h, ms, cnt, len(names)))
+        return {k: (float(ms[i]), int(cnt[i])) for i, k in enumerate(names)}
 
     def selftest_divsqrt(self, n=1 << 27, seed=1):
         a, b = ctypes.c_longlong(0), ctypes.c_longlong(0)

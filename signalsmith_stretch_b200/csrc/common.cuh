@@ -112,13 +112,28 @@ struct Call {
 	int hasRandom;          // some block of the call stretches beyond 2x (:639): the stream takes the k_prep + k_chain path
 	int mapped;             // the stream's parameters need a frequency map or formants: mapped-path kernels, planar spectra
 	int autoPitch;          // formants with the automatic pitch estimate (formant base <= 0): k_pitch takes the stream
-	int nIn, nOut;          // the stream's input / output samples of this call (Ctx::lens, or the call's uniform counts)
+	int nIn, nOut;          // the stream's input / output samples of this call (Ctx::desc, or the call's uniform counts)
+	// the stream's input row, resolved by k_plan: channel c reads in[c*inChan + i].  Every later kernel of the call reads it
+	// here.  The output rows stay the call's (Ctx::out): k_synth2 has no register room for a per-stream row pointer.
+	const float *in;
+	int inChan;
 };
 
-// one stream's sample counts of a per-stream process() call (b200s_process_per_stream)
-struct CallLen {
-	int nIn, nOut;
+// one stream's descriptor of a per-stream call (b200s_run_per_stream; b200s_process_per_stream is every op PROCESS),
+// resolved by the host with the reference's arithmetic
+struct CallDesc {
+	int nIn, nOut; // the stream's counts in the process pass
+	int op;        // B200S_OP_*
+	int pass;      // 1: the process pass takes the stream (PROCESS, OUTPUT_SEEK, FLUSH with outputBlock > 0); 0: absent
+	int seekN;     // SEEK / OUTPUT_SEEK: samples of the seek window (k_seek), at the start of the caller's row
+	int at, tail;  // FLUSH: k_flush_tail's output offset and count (:439-455)
+	float stf;     // SEEK / OUTPUT_SEEK: the seek time factor (:164)
+	// the stream's input row in the process pass (Call::in): PROCESS its caller rows; FLUSH the engine's zero row (inChan
+	// 0); OUTPUT_SEEK its caller rows from seekSamples on (:181)
+	const float *in;
+	int inChan;
 };
+#define B200S_OPBIT(op) (1 << (op))
 
 // one windowed analysis FFT of the call (:333-376): block samples start at stream index `start`
 // (history ++ input), the spectrum goes to row `row` = (2*f + w)*C + c of the stream's `spec` scratch
@@ -182,13 +197,17 @@ struct Ctx {
 	// sub-batch of streams this launch covers (the batch is processed as a few sub-batches on
 	// prioritised CUDA streams so that different kernels of the sequence overlap on the SMs)
 	int sBase, sCount;
-	// I/O of the current call.  nIn / nOut are the uniform counts; with `lens` ([S] {nIn, nOut}, b200s_process_per_stream)
-	// every stream has its own.  Only k_plan reads either: it resolves them into Call::nIn / nOut, which every later kernel
-	// of the call reads.  outTail > 0 (per-stream calls): output samples from Call::nOut up to outTail are written as zero.
+	// I/O of the current call.  nIn / nOut and the rows in / out with their strides are the uniform call's; with `desc` ([S],
+	// b200s_run_per_stream) every stream has its own.  In the process pass only k_plan reads either: it resolves them into
+	// Call::nIn / nOut / in / out, which every later kernel of the call reads.  A stream whose CallDesc::pass is not `pass` is
+	// absent from the process pass.  The phase kernels (k_reset_stft, k_reset_bands, k_seek, k_flush_tail, k_add_output)
+	// take, with `desc`, only the streams whose op is in `opMask`, and in / out here are the caller's rows.
+	// outTail > 0 (per-stream calls): output samples from Call::nOut up to outTail are written as zero.
 	const float *in;
 	float *out;
 	int nIn, nOut;
-	const CallLen *lens;
+	const CallDesc *desc;
+	int pass, opMask;
 	int outTail;
 	long long inStreamStride, outStreamStride; // floats between streams
 	int inChanStride, outChanStride;           // floats between channels

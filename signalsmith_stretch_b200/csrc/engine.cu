@@ -66,13 +66,15 @@ struct b200s_engine {
 	cudaEvent_t evBegin = 0, evSubDone[kMaxSub] = {};
 	int chainedGroups = 0; // > 0: the last operation was a host-buffer process() over this many stream groups (see process_impl)
 	int chainedIn = -1, chainedOut = -1; // its per-channel sample counts (strides): the groups' slabs of the staging buffers sit at sBase*C*n
-	// per-stream sample counts (b200s_process_per_stream): the device table Ctx::lens [S], allocated at configure, and two
-	// pinned staging copies.  Each stream group copies its own slice on its own CUDA stream ahead of its k_plan, so chained
-	// calls need no join for it; a staging copy is rewritten once every group's copy issued from it two calls ago has run.
-	CallLen *dLens = 0;
-	CallLen *pinLens[2] = {0, 0};
-	cudaEvent_t evLens[2][kMaxSub] = {};
-	int lensSlot = 0;
+	// per-stream call descriptors (b200s_run_per_stream): the device table Ctx::desc [S], allocated at configure, and two
+	// pinned staging copies.  In a call of PROCESS / SKIP ops each stream group copies its own slice on its own CUDA stream
+	// ahead of its k_plan, so chained calls need no join for it; a call with a pre or post phase copies the whole table on
+	// the main stream.  A staging copy is rewritten once every copy issued from it two calls ago has run.
+	CallDesc *dDesc = 0;
+	CallDesc *pinDesc[2] = {0, 0};
+	cudaEvent_t evDesc[2][kMaxSub] = {};
+	int descSlot = 0;
+	std::vector<int> allProcess; // [S] B200S_OP_PROCESS: b200s_process_per_stream's ops
 	int chainV = 0, fftV1 = 0; // b200s_set_tuning overrides (0 = default)
 	int exactMath = 0;         // b200s_set_tuning key 3: 1 = the phase chain in the reference's unfused IEEE arithmetic
 	// host-buffer API: stream groups whose H2D copy / kernels / D2H copy are pipelined.  H100 SXM, batch 1024 stereo, one run
@@ -254,7 +256,8 @@ static size_t smem_analyse(const Cfg &g) { return sizeof(float2) * 2 * fft_buf_l
 static size_t smem_prep(const Cfg &g, bool formants = true) { return sizeof(float) * ((formants ? 7 : 6) * (size_t)g.K + 8); }
 static size_t smem_synth(const Cfg &g) { return sizeof(float2) * 2 * fft_buf_len(g.K) + sizeof(float) * 2 * g.pendLen; }
 
-enum { PK_PLAN = 0, PK_ANALYSE, PK_PREP, PK_CHAIN, PK_SYNTH, PK_COMMIT, PK_COUNT };
+// PK_PHASE: the pre and post phases of b200s_run_per_stream (reported when the caller's arrays have room for it)
+enum { PK_PLAN = 0, PK_ANALYSE, PK_PREP, PK_CHAIN, PK_SYNTH, PK_COMMIT, PK_PHASE, PK_COUNT };
 static int prof_mark(b200s_engine *e, int kind, bool begin) {
 	if (!e->profiling) return 0;
 	cudaEvent_t ev;
@@ -659,7 +662,7 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 		if ((rc = dalloc(e, &e->dSprm, (size_t)g.S))) return rc;
 		e->sprmDirty = true;
 	}
-	if (!e->dLens && (rc = dalloc(e, &e->dLens, (size_t)g.S))) return rc; // per-stream sample counts (filled by every per-stream call)
+	if (!e->dDesc && (rc = dalloc(e, &e->dDesc, (size_t)g.S))) return rc; // per-stream call descriptors (filled by every per-stream call)
 
 	// ---- state
 	const size_t SC = (size_t)g.S * g.C;
@@ -828,19 +831,21 @@ static int ensure_buf(b200s_engine *e, float **p, size_t *cap, size_t n, bool ze
 // hIn / hOut (host-buffer API only): packed [S][C][n] host arrays mirrored by dIn / dOut; each stream group
 // then copies its own slab in, runs its kernels and copies its slab out on its own CUDA stream, so that the
 // PCIe transfers of one group overlap the kernels of the others.
-// lenIn / lenOut (b200s_process_per_stream, validated by the caller): host arrays of S per-stream sample counts; nIn / nOut
-// are then the rows' strides, stream s reads lenIn[s] samples of each row and writes lenOut[s], zeros up to the stride.
-// Without them every stream reads nIn and writes nOut.
+// desc (b200s_run_per_stream, resolved by run_impl): the host copy of the call's S descriptors; the streams whose
+// CallDesc::pass is `pass` take part, stream s reading desc[s].nIn samples of each row and writing desc[s].nOut, then zeros
+// up to outTail; every other stream is absent from the pass (but for zeros up to outTail in its row).  nIn / nOut are then
+// the rows' strides.  descSlot >= 0: the stream groups upload their slices of the table from pinDesc[descSlot]; -1: the
+// caller has uploaded the whole table on the main stream.  Without desc every stream reads nIn and writes nOut.
 static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, long long inStreamStride, int nIn,
                         float *dOut, int outChanStride, long long outStreamStride, int nOut,
                         const float *hIn = nullptr, float *hOut = nullptr, const short *hIn16 = nullptr, short *hOut16 = nullptr,
-                        const int *lenIn = nullptr, const int *lenOut = nullptr) {
+                        const CallDesc *desc = nullptr, int pass = 0, int descSlot = -1, int outTail = 0) {
 	const Cfg &g = e->cfg;
 	if (nIn < 0 || nOut < 0) {
 		e->err = "process: negative sample count";
 		return B200S_EINVAL;
 	}
-	const bool perStream = lenIn && lenOut;
+	const bool perStream = desc != nullptr;
 	// the host's decisions over the streams' counts: the longest output sizes the scratch and the grids; a call may need the
 	// random path when ANY stream may stretch beyond 2x; bulk-copy staging needs every input length a multiple of 4
 	int maxOut = nOut;
@@ -849,10 +854,13 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 		maxOut = 0;
 		lowRatio = false;
 		for (int s = 0; s < g.S; ++s) {
-			maxOut = std::max(maxOut, lenOut[s]);
-			if (lenOut[s] > 0) lowRatio = lowRatio || (long long)lenIn[s] * 2 * g.H < (long long)lenOut[s] * (g.H + 4);
+			const bool in = desc[s].pass == pass;
+			const int li = in ? desc[s].nIn : 0, lo = in ? desc[s].nOut : 0;
+			maxOut = std::max(maxOut, lo);
+			if (lo > 0) lowRatio = lowRatio || (long long)li * 2 * g.H < (long long)lo * (g.H + 4);
 			else anyIdle = true;
-			lensAligned = lensAligned && lenIn[s] % 4 == 0;
+			// (an output seek's rows start at its seek window's end: bulk copies need it 16-byte aligned too)
+			lensAligned = lensAligned && li % 4 == 0 && (!in || ((uintptr_t)desc[s].in % 16 == 0 && desc[s].inChan % 4 == 0));
 		}
 	}
 	int rc;
@@ -896,13 +904,10 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	x.outChanStride = outChanStride; x.outStreamStride = outStreamStride;
 	x.inAligned = ((uintptr_t)dIn % 16 == 0) && inChanStride % 4 == 0 && inStreamStride % 4 == 0 && lensAligned && g.histLen % 4 == 0;
 	const int F = frames_bound(g, maxOut);
-	int lk = 0;
-	if (perStream) { // this call's counts into a staging copy; the stream groups upload their slices below
-		lk = e->lensSlot ^= 1;
-		for (int i = 0; i < b200s_engine::kMaxSub; ++i) CK(cudaEventSynchronize(e->evLens[lk][i]));
-		for (int s = 0; s < g.S; ++s) e->pinLens[lk][s] = CallLen{lenIn[s], lenOut[s]};
-		x.lens = e->dLens;
-		x.outTail = nOut;
+	if (perStream) {
+		x.desc = e->dDesc;
+		x.pass = pass;
+		x.outTail = outTail;
 	}
 	// Sub-batch pipeline: the streams of the batch are independent, so the launch sequence is issued
 	// per sub-batch on its own CUDA stream (descending priority).  Sub-batch 0's chain then runs while
@@ -935,9 +940,9 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 		if (nSub > 1 && !chained) CK(cudaStreamWaitEvent(st, e->evBegin, 0));
 		x.sBase = (int)((long long)g.S * sub / nSub);
 		x.sCount = (int)((long long)g.S * (sub + 1) / nSub) - x.sBase;
-		if (perStream) { // the group's slice of the counts, ordered before its k_plan and after its previous call's kernels
-			CK(cudaMemcpyAsync(e->dLens + x.sBase, e->pinLens[lk] + x.sBase, sizeof(CallLen) * x.sCount, cudaMemcpyHostToDevice, st));
-			CK(cudaEventRecord(e->evLens[lk][sub], st));
+		if (perStream && descSlot >= 0) { // the group's slice of the table, ordered before its k_plan and after its previous call's kernels
+			CK(cudaMemcpyAsync(e->dDesc + x.sBase, e->pinDesc[descSlot] + x.sBase, sizeof(CallDesc) * x.sCount, cudaMemcpyHostToDevice, st));
+			CK(cudaEventRecord(e->evDesc[descSlot][sub], st));
 		}
 		if (hIn && nIn > 0)
 			CK(cudaMemcpyAsync((float *)dIn + (size_t)x.sBase * g.C * nIn, hIn + (size_t)x.sBase * g.C * nIn, sizeof(float) * (size_t)x.sCount * g.C * nIn, cudaMemcpyHostToDevice, st));
@@ -1100,6 +1105,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	return 0;
 }
 
+static float seek_time_factor(const Cfg &g, double playbackRate) { return (playbackRate * g.H > 1) ? float(1 / playbackRate) : float(g.H); } // :164
 static int seek_impl(b200s_engine *e, const float *dIn, int chanStride, long long streamStride, int n, double playbackRate, const double *rates = nullptr,
                      const long long *bankEnds = nullptr, long long bankLen = 0) {
 	const Cfg &g = e->cfg;
@@ -1113,7 +1119,7 @@ static int seek_impl(b200s_engine *e, const float *dIn, int chanStride, long lon
 		x.seekEnd = e->dSeekEnd;
 		x.bankLen = bankLen;
 	}
-	float stf = (playbackRate * g.H > 1) ? float(1 / playbackRate) : float(g.H); // :164
+	float stf = seek_time_factor(g, playbackRate);
 	e->seekMayRandom = stf > 1.9f; // the next block takes this as its time factor (:312)
 	if (rates) { // one playback rate per stream (a server whose streams follow their own time maps)
 		int rc;
@@ -1121,7 +1127,7 @@ static int seek_impl(b200s_engine *e, const float *dIn, int chanStride, long lon
 		e->hSeekStf.resize(g.S);
 		e->seekMayRandom = false;
 		for (int s = 0; s < g.S; ++s) {
-			e->hSeekStf[s] = (rates[s] * g.H > 1) ? float(1 / rates[s]) : float(g.H);
+			e->hSeekStf[s] = seek_time_factor(g, rates[s]);
 			if (e->hSeekStf[s] > 1.9f) e->seekMayRandom = true;
 		}
 		CK(cudaMemcpyAsync(e->dSeekStf, e->hSeekStf.data(), sizeof(float) * g.S, cudaMemcpyHostToDevice, e->stream));
@@ -1167,7 +1173,7 @@ static int output_seek_impl(b200s_engine *e, const float *dIn, int chanStride, l
 	if ((rc = ensure_buf(e, &e->dTmp, &e->tmpCap, tn, false))) return rc;
 	if ((rc = process_impl(e, dIn + seekSamples, chanStride, streamStride, surplus, e->dTmp, outLat, (long long)g.C * outLat, outLat))) return rc; // :196
 	Ctx x = make_ctx(e);
-	B200S_LAUNCH(k_add_output, dim3(g.C, g.S), dim3(kThreads), 0, e->stream, x, e->dTmp, outLat); // :199-203
+	B200S_LAUNCH(k_add_output, dim3(g.C, g.S), dim3(kThreads), 0, e->stream, x, (const float *)e->dTmp, outLat); // :199-203
 	CKL();
 	return 0;
 }
@@ -1186,6 +1192,159 @@ static int stage_out(b200s_engine *e, int n) {
 static int fetch_out(b200s_engine *e, float *out, int n) {
 	if (n > 0) CK(cudaMemcpyAsync(out, e->dOut, sizeof(float) * (size_t)e->cfg.S * e->cfg.C * n, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
+	return 0;
+}
+
+// b200s_run_per_stream (arguments validated by check_run): every stream runs its own op, in three phases (DESIGN.md §3.11).
+//   pre:     RESET / OUTPUT_SEEK: the full reset (:175), then SEEK / OUTPUT_SEEK: k_seek with the stream's window and factor
+//   process: ONE process_impl pass over the PROCESS, OUTPUT_SEEK (:196) and FLUSH (:440-441) streams, each on its own rows
+//            (CallDesc::in / out, resolved into Call by k_plan): a FLUSH stream reads the engine's zero row, an OUTPUT_SEEK
+//            stream its caller rows after the seek window and writes its pre-roll into dTmp [S][C][outputLatency]
+//   post:    FLUSH: k_flush_tail and the flush's reset (:442-463); OUTPUT_SEEK: k_add_output from dTmp (:198-203)
+// Every other stream is absent from the pass (k_plan), so its state is untouched and k_commit copies its history
+// unchanged into the other buffer.  A phase that no stream needs is not launched.  Host buffers: a call of PROCESS / SKIP
+// ops with some PROCESS pipelines its stream groups as b200s_process_async does; any other call copies the input slab in
+// on the main stream, runs on the device and copies the output slab back.
+static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStride, const int *nIn, float *out, int outStride,
+                    const int *nOut, const double *rates, bool host, bool wait) {
+	const Cfg &g = e->cfg;
+	const long long C = g.C;
+	const int inLat = g.B - g.B / 2, outLat = g.B / 2 + (g.split ? g.H : 0);
+	int opsUsed = 0, zeroLen = 0;
+	for (int s = 0; s < g.S; ++s) {
+		opsUsed |= B200S_OPBIT(ops[s]);
+		if (ops[s] == B200S_OP_FLUSH) {
+			const int outputBlock = std::max(0, nOut[s] - g.H); // :439
+			zeroLen = std::max(zeroLen, std::max(0, int(outputBlock * (rates ? float(rates[s]) : 0.f)))); // :440
+		}
+	}
+	const int preOps = B200S_OPBIT(B200S_OP_RESET) | B200S_OPBIT(B200S_OP_SEEK) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
+	const int postOps = B200S_OPBIT(B200S_OP_FLUSH) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
+	const bool phases = (opsUsed & (preOps | postOps)) != 0;
+	int rc;
+	// buffers first (growing one synchronises and may move it): the descriptors below hold their addresses
+	if (host) {
+		if ((size_t)C * g.S * std::max(inStride, 1) > e->inCap || (size_t)C * g.S * std::max(outStride, 1) > e->outCap || !e->dIn || !e->dOut) {
+			// growing the staging buffers would invalidate copies still in flight: drain first
+			CK(cudaStreamSynchronize(e->stream));
+		}
+		if ((rc = stage_in(e, nullptr, inStride))) return rc; // capacity only
+		if ((rc = stage_out(e, outStride))) return rc;
+	}
+	// (sized by b200s_reserve: no allocation then)
+	if ((opsUsed & B200S_OPBIT(B200S_OP_FLUSH)) && (rc = ensure_buf(e, &e->dZero, &e->zeroCap, (size_t)std::max(zeroLen, 1), true))) return rc;
+	// An output seek writes outputLatency samples of pre-roll into its output rows, which k_add_output reads back and then
+	// zeroes.  Rows narrower than that: the pass writes into dTmp [S][C][outputLatency], copied back to the caller's rows.
+	const int W = (opsUsed & B200S_OPBIT(B200S_OP_OUTPUT_SEEK)) ? std::max(outStride, outLat) : outStride;
+	if (W > outStride && (rc = ensure_buf(e, &e->dTmp, &e->tmpCap, (size_t)g.S * C * W, false))) return rc;
+	const float *dIn = host ? e->dIn : in;
+	float *dOut = host ? e->dOut : out, *pOut = W > outStride ? e->dTmp : dOut;
+	const int lk = e->descSlot ^= 1;
+	for (int i = 0; i < b200s_engine::kMaxSub; ++i) CK(cudaEventSynchronize(e->evDesc[lk][i]));
+	CallDesc *d = e->pinDesc[lk];
+	bool anyPass = false, seekSlow = false;
+	for (int s = 0; s < g.S; ++s) {
+		CallDesc c;
+		memset(&c, 0, sizeof(c));
+		c.op = ops[s];
+		c.in = dIn + (size_t)s * C * inStride;
+		c.inChan = inStride;
+		switch (c.op) {
+		case B200S_OP_PROCESS:
+			c.pass = 1;
+			c.nIn = nIn[s];
+			c.nOut = nOut[s];
+			break;
+		case B200S_OP_SEEK:
+			c.seekN = nIn[s];
+			c.stf = seek_time_factor(g, rates[s]);
+			break;
+		case B200S_OP_OUTPUT_SEEK: {
+			const int surplus = std::max(nIn[s] - inLat, 0); // :177
+			const float rate = surplus / float(outLat);      // :178
+			c.seekN = nIn[s] - surplus;                      // :181
+			c.stf = seek_time_factor(g, rate);
+			c.pass = 1;
+			c.nIn = surplus;
+			c.nOut = outLat;
+			c.in += c.seekN;
+			break;
+		}
+		case B200S_OP_FLUSH: {
+			const float rate = rates ? float(rates[s]) : 0.f;
+			const int outputBlock = std::max(0, nOut[s] - g.H); // :439
+			if (outputBlock > 0) {
+				c.pass = 1;
+				c.nIn = std::max(0, int(outputBlock * rate)); // :440
+				c.nOut = outputBlock;
+				c.in = e->dZero;
+				c.inChan = 0;
+			}
+			c.at = outputBlock;
+			c.tail = nOut[s] - outputBlock;
+			break;
+		}
+		default: break; // RESET, SKIP
+		}
+		anyPass = anyPass || c.pass;
+		seekSlow = seekSlow || c.stf > 1.9f;
+		d[s] = c;
+	}
+	if (host && !phases && anyPass) { // the stream groups copy their own slabs in and out
+		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, d, 1, lk, outStride))) return rc;
+		if (wait) CK(cudaStreamSynchronize(e->stream));
+		return 0;
+	}
+	if (host) {
+		e->chainedGroups = 0;
+		if (in && inStride > 0) CK(cudaMemcpyAsync(e->dIn, in, sizeof(float) * (size_t)g.S * C * inStride, cudaMemcpyHostToDevice, e->stream));
+	}
+	if (phases) { // the whole table on the main stream, ahead of the pre phase (the call joins)
+		e->chainedGroups = 0;
+		CK(cudaMemcpyAsync(e->dDesc, d, sizeof(CallDesc) * g.S, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaEventRecord(e->evDesc[lk][0], e->stream));
+	}
+	Ctx x = make_ctx(e);
+	x.desc = e->dDesc;
+	x.in = dIn; x.inChanStride = inStride; x.inStreamStride = C * inStride;
+	if (opsUsed & preOps) {
+		if (opsUsed & (B200S_OPBIT(B200S_OP_RESET) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK))) {
+			x.opMask = B200S_OPBIT(B200S_OP_RESET) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_stft, dim3(g.S), dim3(kThreads), 0, e->stream, x));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_bands, dim3(g.S), dim3(kThreads), 0, e->stream, x, 15));
+		}
+		if (opsUsed & (B200S_OPBIT(B200S_OP_SEEK) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK))) {
+			x.opMask = B200S_OPBIT(B200S_OP_SEEK) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
+			PROF(PK_PHASE, B200S_LAUNCH(k_seek, dim3(g.S), dim3(kThreads), 0, e->stream, x, 0.f));
+			e->seekMayRandom = e->seekMayRandom || seekSlow; // (other streams may still carry an earlier seek's factor)
+		}
+	}
+	if (anyPass) {
+		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, pOut, W, C * W, W, nullptr, nullptr, nullptr, nullptr, d, 1, phases ? -1 : lk, W))) return rc;
+	} else if (W > 0) { // no process pass: every row is zero but for the flushes' tails (post phase)
+		const size_t cnt = (size_t)g.S * C * W;
+		PROF(PK_PHASE, B200S_LAUNCH(k_zero, dim3((unsigned)std::min<size_t>((cnt + 1023) / 1024, 4096)), dim3(256), 0, e->stream, pOut, cnt));
+	}
+	if (opsUsed & postOps) {
+		Ctx y = make_ctx(e); // (after the pass's history flip)
+		y.desc = e->dDesc;
+		y.out = pOut; y.outChanStride = W; y.outStreamStride = C * W;
+		y.outTail = W;
+		if (opsUsed & B200S_OPBIT(B200S_OP_FLUSH)) {
+			y.opMask = B200S_OPBIT(B200S_OP_FLUSH);
+			PROF(PK_PHASE, B200S_LAUNCH(k_flush_tail, dim3(g.C, g.S), dim3(kThreads), sizeof(float) * g.B, e->stream, y, 0, 0));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_stft, dim3(g.S), dim3(kThreads), 0, e->stream, y));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_bands, dim3(g.S), dim3(kThreads), 0, e->stream, y, 6));
+		}
+		if (opsUsed & B200S_OPBIT(B200S_OP_OUTPUT_SEEK)) {
+			y.opMask = B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
+			PROF(PK_PHASE, B200S_LAUNCH(k_add_output, dim3(g.C, g.S), dim3(kThreads), 0, e->stream, y, (const float *)nullptr, outLat));
+		}
+	}
+	if (pOut != dOut && outStride > 0)
+		PROF(PK_PHASE, B200S_LAUNCH(k_copy_rows, dim3((unsigned)std::min<long long>((long long)g.S * C, 65535)), dim3(256), 0, e->stream, dOut, outStride, (const float *)pOut, W, outStride, (int)(g.S * C)));
+	if (host && out && outStride > 0) CK(cudaMemcpyAsync(out, e->dOut, sizeof(float) * (size_t)g.S * C * outStride, cudaMemcpyDeviceToHost, e->stream));
+	if (wait) CK(cudaStreamSynchronize(e->stream));
 	return 0;
 }
 
@@ -1208,6 +1367,7 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 	}
 	b200s_engine *e = new b200s_engine();
 	e->S = batch;
+	e->allProcess.assign((size_t)batch, B200S_OP_PROCESS);
 	e->seed = seed;
 	e->device = device;
 	memset(&e->cfg, 0, sizeof(e->cfg));
@@ -1239,8 +1399,8 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 	for (int k = 0; k < 2; ++k) {
 		bool ok = host_alloc((void **)&e->pinSprm[k], sizeof(StreamParams) * (size_t)batch) &&
 		          cudaEventCreateWithFlags(&e->evSprm[k], cudaEventDisableTiming) == cudaSuccess &&
-		          host_alloc((void **)&e->pinLens[k], sizeof(CallLen) * (size_t)batch);
-		for (int i = 0; i < b200s_engine::kMaxSub && ok; ++i) ok = cudaEventCreateWithFlags(&e->evLens[k][i], cudaEventDisableTiming) == cudaSuccess;
+		          host_alloc((void **)&e->pinDesc[k], sizeof(CallDesc) * (size_t)batch);
+		for (int i = 0; i < b200s_engine::kMaxSub && ok; ++i) ok = cudaEventCreateWithFlags(&e->evDesc[k][i], cudaEventDisableTiming) == cudaSuccess;
 		if (!ok) {
 			g_createError = "pinned host memory / event creation failed";
 			b200s_destroy(e);
@@ -1279,13 +1439,13 @@ void b200s_destroy(b200s_engine *e) {
 	dfree(e->dSeekStf);
 	dfree(e->dSeekEnd);
 	dfree(e->dSprm);
-	dfree(e->dLens);
+	dfree(e->dDesc);
 	for (int k = 0; k < 2; ++k) {
 		host_free(e->pinSprm[k]);
 		if (e->evSprm[k]) cudaEventDestroy(e->evSprm[k]);
-		host_free(e->pinLens[k]);
+		host_free(e->pinDesc[k]);
 		for (int i = 0; i < b200s_engine::kMaxSub; ++i)
-			if (e->evLens[k][i]) cudaEventDestroy(e->evLens[k][i]);
+			if (e->evDesc[k][i]) cudaEventDestroy(e->evDesc[k][i]);
 	}
 	for (int i = 0; i < b200s_engine::kMaxSub; ++i) {
 		if (e->subStream[i]) cudaStreamDestroy(e->subStream[i]);
@@ -1362,12 +1522,19 @@ int b200s_reset(b200s_engine *e) {
 int b200s_reserve(b200s_engine *e, int maxIn, int maxOut) {
 	NEED_CFG();
 	int rc;
-	if ((rc = ensure_scratch(e, maxOut))) return rc;
+	// (an output seek of b200s_run_per_stream writes outputLatency samples of pre-roll in the process pass)
+	const int pass2Out = std::max(maxOut, b200s_output_latency(e));
+	if ((rc = ensure_scratch(e, pass2Out))) return rc;
 	if (e->nMapped > 0 && (rc = e->stepMajor ? ensure_stepmajor(e) : ensure_coef(e))) return rc;
 	if ((rc = stage_in(e, 0, 0))) return rc;
 	size_t ci = (size_t)e->cfg.S * e->cfg.C * std::max(maxIn, 1), co = (size_t)e->cfg.S * e->cfg.C * std::max(maxOut, 1);
 	if ((rc = ensure_buf(e, &e->dIn, &e->inCap, ci, false))) return rc;
-	return ensure_buf(e, &e->dOut, &e->outCap, co, false);
+	if ((rc = ensure_buf(e, &e->dOut, &e->outCap, co, false))) return rc;
+	// b200s_run_per_stream: the zero row of flushes that read up to maxIn zeros; output rows narrower than outputLatency
+	// take the output seeks' pre-roll through dTmp
+	if ((rc = ensure_buf(e, &e->dZero, &e->zeroCap, (size_t)std::max(maxIn, 1), true))) return rc;
+	if (maxOut >= b200s_output_latency(e)) return 0;
+	return ensure_buf(e, &e->dTmp, &e->tmpCap, (size_t)e->cfg.S * e->cfg.C * b200s_output_latency(e), false);
 }
 
 int b200s_batch(const b200s_engine *e) { return e ? e->S : 0; }
@@ -1554,10 +1721,10 @@ int b200s_process_async(b200s_engine *e, const float *in, int nIn, float *out, i
 	if ((rc = stage_out(e, nOut))) return rc;
 	return process_impl(e, e->dIn, nIn, (long long)e->cfg.C * nIn, nIn, e->dOut, nOut, (long long)e->cfg.C * nOut, nOut, in, out);
 }
-// Arguments of the per-stream process calls, checked before anything is enqueued
-static int check_per_stream(b200s_engine *e, const char *fn, int inStride, const int *nIn, int outStride, const int *nOut) {
-	if (!nIn || !nOut) {
-		e->err = std::string(fn) + ": input_samples and output_samples must not be NULL";
+// Arguments of the per-stream calls, checked before anything is enqueued
+static int check_run(b200s_engine *e, const char *fn, const int *ops, int inStride, const int *nIn, int outStride, const int *nOut, const double *rates) {
+	if (!ops || !nIn || !nOut) {
+		e->err = std::string(fn) + ": " + (ops ? "input_samples and output_samples must not be NULL" : "ops must not be NULL");
 		return B200S_EINVAL;
 	}
 	if (inStride < 0 || outStride < 0) {
@@ -1565,45 +1732,53 @@ static int check_per_stream(b200s_engine *e, const char *fn, int inStride, const
 		return B200S_EINVAL;
 	}
 	for (int s = 0; s < e->S; ++s) {
-		const bool badIn = nIn[s] < 0 || nIn[s] > inStride;
-		if (badIn || nOut[s] < 0 || nOut[s] > outStride) {
-			e->err = std::string(fn) + ": stream " + std::to_string(s) + ": " + (badIn ? "input_samples " : "output_samples ") +
-			         std::to_string(badIn ? nIn[s] : nOut[s]) + " is outside [0, " + std::to_string(badIn ? inStride : outStride) + "]";
+		const int op = ops[s];
+		std::string why;
+		if (op < B200S_OP_SKIP || op > B200S_OP_RESET) why = "op " + std::to_string(op) + " is not a B200S_OP_*";
+		else if (op == B200S_OP_SEEK && !rates) why = "SEEK needs playback_rates";
+		else if (nIn[s] != 0 && (op == B200S_OP_FLUSH || op == B200S_OP_RESET || op == B200S_OP_SKIP))
+			why = "op " + std::to_string(op) + " reads no input, input_samples is " + std::to_string(nIn[s]);
+		else if (nOut[s] != 0 && op != B200S_OP_PROCESS && op != B200S_OP_FLUSH)
+			why = "op " + std::to_string(op) + " writes no output, output_samples is " + std::to_string(nOut[s]);
+		else if (nIn[s] < 0 || nIn[s] > inStride)
+			why = "input_samples " + std::to_string(nIn[s]) + " is outside [0, " + std::to_string(inStride) + "]";
+		else if (nOut[s] < 0 || nOut[s] > outStride)
+			why = "output_samples " + std::to_string(nOut[s]) + " is outside [0, " + std::to_string(outStride) + "]";
+		if (!why.empty()) {
+			e->err = std::string(fn) + ": stream " + std::to_string(s) + ": " + why;
 			return B200S_EINVAL;
 		}
 	}
 	return 0;
 }
-int b200s_process_per_stream(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {
+static int run_entry(b200s_engine *e, const char *fn, const int *ops, const float *in, int inStride, const int *nIn, float *out,
+                     int outStride, const int *nOut, const double *rates, bool host, bool wait) {
 	NEED_CFG();
 	int rc;
-	if ((rc = check_per_stream(e, "b200s_process_per_stream", inStride, nIn, outStride, nOut))) return rc;
-	if ((rc = stage_in(e, nullptr, inStride))) return rc; // capacity only: the copies are issued per stream group
-	if ((rc = stage_out(e, outStride))) return rc;
-	const long long C = e->cfg.C;
-	if ((rc = process_impl(e, e->dIn, inStride, C * inStride, inStride, e->dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, nIn, nOut))) return rc;
-	CK(cudaStreamSynchronize(e->stream));
-	return 0;
+	if ((rc = check_run(e, fn, ops, inStride, nIn, outStride, nOut, rates))) return rc;
+	return run_impl(e, ops, in, inStride, nIn, out, outStride, nOut, rates, host, wait);
+}
+int b200s_run_per_stream(b200s_engine *e, const int *ops, const float *in, int inStride, const int *nIn, float *out, int outStride,
+                         const int *nOut, const double *rates) {
+	return run_entry(e, "b200s_run_per_stream", ops, in, inStride, nIn, out, outStride, nOut, rates, true, true);
+}
+int b200s_run_per_stream_async(b200s_engine *e, const int *ops, const float *in, int inStride, const int *nIn, float *out, int outStride,
+                               const int *nOut, const double *rates) {
+	return run_entry(e, "b200s_run_per_stream_async", ops, in, inStride, nIn, out, outStride, nOut, rates, true, false);
+}
+int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *dIn, int inStride, const int *nIn, float *dOut, int outStride,
+                                const int *nOut, const double *rates) {
+	return run_entry(e, "b200s_run_per_stream_device", ops, dIn, inStride, nIn, dOut, outStride, nOut, rates, false, false);
+}
+// process() with per-stream lengths: b200s_run_per_stream with every op PROCESS
+int b200s_process_per_stream(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {
+	return run_entry(e, "b200s_process_per_stream", e ? e->allProcess.data() : nullptr, in, inStride, nIn, out, outStride, nOut, nullptr, true, true);
 }
 int b200s_process_per_stream_async(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {
-	NEED_CFG();
-	int rc;
-	if ((rc = check_per_stream(e, "b200s_process_per_stream_async", inStride, nIn, outStride, nOut))) return rc;
-	if ((size_t)e->cfg.S * e->cfg.C * std::max(inStride, 1) > e->inCap || (size_t)e->cfg.S * e->cfg.C * std::max(outStride, 1) > e->outCap || !e->dIn || !e->dOut) {
-		// growing the staging buffers would invalidate copies still in flight: drain first
-		CK(cudaStreamSynchronize(e->stream));
-	}
-	if ((rc = stage_in(e, nullptr, inStride))) return rc;
-	if ((rc = stage_out(e, outStride))) return rc;
-	const long long C = e->cfg.C;
-	return process_impl(e, e->dIn, inStride, C * inStride, inStride, e->dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, nIn, nOut);
+	return run_entry(e, "b200s_process_per_stream_async", e ? e->allProcess.data() : nullptr, in, inStride, nIn, out, outStride, nOut, nullptr, true, false);
 }
 int b200s_process_per_stream_device(b200s_engine *e, const float *dIn, int inStride, const int *nIn, float *dOut, int outStride, const int *nOut) {
-	NEED_CFG();
-	int rc;
-	if ((rc = check_per_stream(e, "b200s_process_per_stream_device", inStride, nIn, outStride, nOut))) return rc;
-	const long long C = e->cfg.C;
-	return process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, nullptr, nullptr, nullptr, nullptr, nIn, nOut);
+	return run_entry(e, "b200s_process_per_stream_device", e ? e->allProcess.data() : nullptr, dIn, inStride, nIn, dOut, outStride, nOut, nullptr, false, false);
 }
 int b200s_flush(b200s_engine *e, float *out, int nOut, float rate) {
 	NEED_CFG();
@@ -1671,7 +1846,7 @@ int b200s_profile_begin(b200s_engine *e) {
 	return 0;
 }
 int b200s_profile_end(b200s_engine *e, float *ms, int *counts, int n) {
-	if (!e || !ms || !counts || n < PK_COUNT) return B200S_EINVAL;
+	if (!e || !ms || !counts || n < PK_PHASE) return B200S_EINVAL;
 	e->profiling = false;
 	CK(cudaStreamSynchronize(e->stream));
 	for (int i = 0; i < n; ++i) {
@@ -1680,6 +1855,7 @@ int b200s_profile_end(b200s_engine *e, float *ms, int *counts, int n) {
 	}
 	for (size_t i = 0; i < e->profKind.size(); ++i) {
 		float t = 0;
+		if (e->profKind[i] >= n) continue; // (the phases' kind, when the caller asked for the six kernels only)
 		CK(cudaEventElapsedTime(&t, e->profEv[2 * i], e->profEv[2 * i + 1]));
 		ms[e->profKind[i]] += t;
 		counts[e->profKind[i]] += 1;

@@ -56,7 +56,9 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	const long long total = (long long)x.sCount * PJ;
 
 	struct Item {
-		int s, hasB, nIn; // nIn: the stream's Call::nIn (loaded with the descriptors, off the staging path)
+		int s, hasB, nIn; // nIn, in, inChan: the stream's Call (loaded with the descriptors, off the staging path)
+		const float *in;
+		int inChan;
 		Job a, b;
 	};
 	// item -> jobs; false when the stream has fewer pairs than slots
@@ -68,6 +70,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 		const Job *jb = x.jobs + (size_t)m.s * 2 * g.C * x.maxFrames + 2 * (int)(it % PJ);
 		m.hasB = x.call[m.s].nJobs;
 		m.nIn = x.call[m.s].nIn;
+		m.in = x.call[m.s].in;
+		m.inChan = x.call[m.s].inChan;
 		m.a = jb[0];
 		m.b = jb[1];
 	};
@@ -96,8 +100,9 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	fence_async_proxy();
 	__syncthreads();
 	unsigned stagePar = 0u;
-	auto stage_job = [&](float *st, int s, int nIn, const Job &j, int t0, int nT) {
-		const float *ib = x.in + (size_t)s * x.inStreamStride + (size_t)j.c * x.inChanStride;
+	auto stage_job = [&](float *st, const Item &m, const Job &j, int t0, int nT) {
+		const int s = m.s, nIn = m.nIn;
+		const float *ib = m.in + (size_t)j.c * m.inChan;
 		const float *he = x.histCur + ((size_t)s * g.C + j.c) * g.histLen + g.histLen;
 		if (x.inAligned) {
 			const int sh = j.start & 3, a00 = j.start - sh, nCh = (B + sh + 3) >> 2;
@@ -127,8 +132,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	Item cur, nxt;
 	long long item = next_valid(blockIdx.x, cur);
 	if (item < total) {
-		stage_job(stA, cur.s, cur.nIn, cur.a, 0, 256);
-		stage_job(stB, cur.s, cur.nIn, cur.b, 32, 256);
+		stage_job(stA, cur, cur.a, 0, 256);
+		stage_job(stB, cur, cur.b, 32, 256);
 	}
 	long long nitem = item < total ? next_valid(item + gridDim.x, nxt) : total;
 	while (item < total) {
@@ -179,8 +184,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 			item = nitem;
 			cur = nxt;
 			if (item < total) {
-				stage_job(stA, cur.s, cur.nIn, cur.a, 0, 256);
-				stage_job(stB, cur.s, cur.nIn, cur.b, 32, 256);
+				stage_job(stA, cur, cur.a, 0, 256);
+				stage_job(stB, cur, cur.b, 32, 256);
 				nitem = next_valid(item + gridDim.x, nxt);
 			}
 			continue;
@@ -216,8 +221,8 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 			}
 		}
 		if (nitem < total) { // start the next pair's input on its way while this FFT runs
-			stage_job(stA, nxt.s, nxt.nIn, nxt.a, 0, 256);
-			stage_job(stB, nxt.s, nxt.nIn, nxt.b, 32, 256);
+			stage_job(stA, nxt, nxt.a, 0, 256);
+			stage_job(stB, nxt, nxt.b, 32, 256);
 			if (cand < total) fetch_raw(cand, n2); // descriptor of the item after next: loads in flight until the end of the iteration
 		}
 		if constexpr (PROBE != 4) pair_dit_stage_b<KT>(buf, tw, tid);
@@ -314,7 +319,7 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 	const Call cl = x.call[s];
 	float *out = x.out + (size_t)s * x.outStreamStride + (size_t)c * x.outChanStride;
 	if (cl.bypass) { // :252-267
-		const float *in = x.in + (size_t)s * x.inStreamStride + (size_t)c * x.inChanStride;
+		const float *in = cl.in + (size_t)c * cl.inChan;
 		for (int i = tid; i < cl.nOut; i += 256) out[i] = cl.nIn > 0 ? in[i % cl.nIn] : 0.f;
 		for (int i = cl.nOut + tid; i < x.outTail; i += 256) out[i] = 0.f;
 		return;
