@@ -188,6 +188,45 @@ int b200s_run_per_stream_async(b200s_engine *e, const int *ops, const float *in,
 int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *d_in, int in_stride, const int *input_samples,
                                 float *d_out, int out_stride, const int *output_samples, const double *playback_rates);
 
+/* ---- moving, duplicating and saving single streams ----
+ * A server that rebalances streams over engines or GPUs, forks a session to preview two settings from the same point,
+ * or checkpoints a session into another process moves one stream's complete state: history, pending output and its
+ * windowProducts, the input / prevInput / output spectra and the prediction energy, the block scheduler, the random
+ * engine, the pitch smoother and the stream's parameters.
+ *
+ * b200s_copy_streams: afterwards stream dst_streams[i] of `dst` is what a reference object is after
+ * `*dst_i = *src_i` (member-wise copy); the source is unchanged, byte for byte.  Fed the same calls, the source and the
+ * copy then give bit-identical outputs, each equal to a one-stream reference driven through that stream's whole history.
+ *   - Every source is read before any destination is written: swaps and rotations within one engine work, and one
+ *     source may go to several destinations.  Duplicate destinations are refused.
+ *   - src == dst is allowed; src and dst may be different handles on the same or on different devices.  Both must have
+ *     the same configuration (channels, block, interval, split); batch, seed and tuning keys may differ (exact math,
+ *     key 3, included: the copy continues in the destination's arithmetic).
+ *   - The frequency-map table is one per engine.  Within one engine a stream's use of it is copied as it is; a stream
+ *     that uses it (set by b200s_set_freq_map_table with n > 0 and not cleared since) may only go to another engine whose
+ *     table is bit-identical.  A stream that does not use it arrives not using the destination's.
+ *   - The parameters copied are the source's current ones (a setter called just before is included).  Whether the next
+ *     call may need the random path (stretch beyond 2x, a slow seek) travels with the stream.
+ *   - Ordering: the call acts as if it ran at its place in both handles' stream orders.  It enqueues without a host
+ *     synchronisation, like the *_device calls (also after chained asynchronous host-buffer calls); later calls on either
+ *     handle see the result.  n == 0 enqueues nothing.
+ * b200s_export_streams writes n records of b200s_stream_state_bytes(e) bytes to host memory (synchronous);
+ * b200s_import_streams reads them into the listed slots (synchronous).  A record starts with a header (magic, format
+ * version, configuration, the stream's parameters and a fingerprint of the map table it uses); import checks every
+ * header against the engine before anything is enqueued.  Records are in the host's byte order.
+ * b200s_clone: a new handle with the same batch, device, seed, configuration, tuning keys, parameters, map table and
+ * state of every stream (an unconfigured source gives an unconfigured clone).  The copy members of the C++ facade.
+ * B200S_EINVAL before anything is enqueued, b200s_last_error() naming the first offending entry (for a copy on both
+ * handles): NULL arrays with n > 0, n < 0, an index outside [0, batch), duplicate destinations, an unconfigured engine,
+ * a configuration mismatch, a bad record header, a map-table mismatch.
+ * Copies and imports stage through device buffers that grow on first use (b200s_device_allocations counts them); a
+ * later call with at most as many streams allocates nothing. */
+int b200s_stream_state_bytes(const b200s_engine *e); /* bytes of one stream's record; B200S_EINVAL if not configured */
+int b200s_copy_streams(b200s_engine *dst, const int *dst_streams, b200s_engine *src, const int *src_streams, int n);
+int b200s_export_streams(b200s_engine *e, const int *streams, int n, void *host_dst);
+int b200s_import_streams(b200s_engine *e, const int *streams, int n, const void *host_src);
+int b200s_clone(b200s_engine *src, b200s_engine **out);
+
 /* ---- measurement helpers (no reference equivalent; used by bench.py) ---- */
 /* CUDA events recorded on the handle's stream around whatever is enqueued in between. */
 int b200s_timer_start(b200s_engine *e);

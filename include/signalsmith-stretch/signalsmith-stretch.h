@@ -29,6 +29,7 @@
 #include <functional>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../b200_stretch.h"
@@ -43,8 +44,26 @@ struct SignalsmithStretch {
 	SignalsmithStretch() : SignalsmithStretch(0) {}
 	SignalsmithStretch(long seed) { check(b200s_create(1, seed, 0, &engine)); } // :38-39
 	~SignalsmithStretch() { b200s_destroy(engine); }
-	SignalsmithStretch(const SignalsmithStretch &) = delete;
-	SignalsmithStretch &operator=(const SignalsmithStretch &) = delete;
+	// Copyable and movable like the reference class (whose members the compiler copies): a copy continues exactly where
+	// the original is -- parameters, state and random engine (b200s_clone).  A moved-from object holds no engine.
+	SignalsmithStretch(const SignalsmithStretch &other) : channels(other.channels) {
+		if (other.engine) check(b200s_clone(other.engine, &engine));
+	}
+	SignalsmithStretch &operator=(const SignalsmithStretch &other) {
+		if (this != &other) {
+			SignalsmithStretch copy(other);
+			swap(copy);
+		}
+		return *this;
+	}
+	SignalsmithStretch(SignalsmithStretch &&other) noexcept { swap(other); }
+	SignalsmithStretch &operator=(SignalsmithStretch &&other) noexcept {
+		if (this != &other) {
+			SignalsmithStretch gone(std::move(*this));
+			swap(other);
+		}
+		return *this;
+	}
 
 	int inputLatency() const { return b200s_input_latency(engine); }   // :42
 	int outputLatency() const { return b200s_output_latency(engine); } // :45
@@ -136,6 +155,14 @@ private:
 	std::string error;
 
 	bool failed = false; // soft-error mode: the last call failed, scatter() writes zeros
+	void swap(SignalsmithStretch &other) noexcept {
+		std::swap(engine, other.engine);
+		std::swap(channels, other.channels);
+		stageIn.swap(other.stageIn);
+		stageOut.swap(other.stageOut);
+		error.swap(other.error);
+		std::swap(failed, other.failed);
+	}
 	void check(int rc) {
 		failed = rc != 0;
 		if (!failed) return;

@@ -37,6 +37,7 @@ ABI_SYMBOLS = [
     "b200s_timer_start", "b200s_timer_stop", "b200s_kernel_launches", "b200s_device_allocations", "b200s_unserved_random_blocks", "b200s_profile_begin", "b200s_profile_end",
     "b200s_selftest_divsqrt",
     "b200s_state_size", "b200s_get_state", "b200s_set_state",
+    "b200s_stream_state_bytes", "b200s_copy_streams", "b200s_export_streams", "b200s_import_streams", "b200s_clone",
 ]
 
 STATE = {"input": 0, "prevInput": 1, "output": 2, "predEnergy": 4, "history": 20, "pending": 21, "pendingWp": 22}
@@ -56,7 +57,7 @@ def build_library(verbose=False):
 
     src = os.path.join(_HERE, "csrc", "engine.cu")
     out = library_path()
-    deps = [src] + [os.path.join(_HERE, "csrc", f) for f in ("kernels.cuh", "fft.cuh", "common.cuh", "chain_direct.cuh", "chain_direct2.cuh", "fft2.cuh", "stft2.cuh", "chain_direct3.cuh", "chain_direct4.cuh", "chain_ws.cuh", "chain_t.cuh", "chain_direct6.cuh")]
+    deps = [src] + [os.path.join(_HERE, "csrc", f) for f in ("kernels.cuh", "fft.cuh", "common.cuh", "chain_direct.cuh", "chain_direct2.cuh", "fft2.cuh", "stft2.cuh", "chain_direct3.cuh", "chain_direct4.cuh", "chain_ws.cuh", "chain_t.cuh", "chain_direct6.cuh", "state_copy.cuh")]
     deps.append(os.path.join(_ROOT, "include", "b200_stretch.h"))
     deps.append(os.path.abspath(__file__))  # the nvcc command line below
     if os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps):
@@ -109,6 +110,9 @@ def _bind(lib):
         "b200s_profile_begin": (ci, [vp]), "b200s_profile_end": (ci, [vp, fp, ip, ci]),
         "b200s_selftest_divsqrt": (ci, [vp, cll, cll, ctypes.POINTER(cll), ctypes.POINTER(cll)]),
         "b200s_state_size": (ci, [vp, ci]), "b200s_get_state": (ci, [vp, ci, vp]), "b200s_set_state": (ci, [vp, ci, vp]),
+        "b200s_stream_state_bytes": (ci, [vp]), "b200s_copy_streams": (ci, [vp, ip, vp, ip, ci]),
+        "b200s_export_streams": (ci, [vp, ip, ci, vp]), "b200s_import_streams": (ci, [vp, ip, ci, vp]),
+        "b200s_clone": (ci, [vp, ctypes.POINTER(vp)]),
     }
     for name in ("batch", "channels", "block_samples", "interval_samples", "input_latency", "output_latency",
                  "split_computation", "seek_length", "fft_samples", "bands"):
@@ -486,6 +490,54 @@ class BatchStretch:
         ok = ctypes.c_int(0)
         self._ck(self._lib.b200s_exact(self._h, x.ctypes.data, n_in, out.ctypes.data, outputSamples, ctypes.byref(ok)))
         return bool(ok.value), out
+
+    # ---- moving, duplicating and saving single streams (b200s_copy_streams / _export_streams / _import_streams / _clone) ----
+    def _stream_list(self, streams, name):
+        a = np.ascontiguousarray(np.atleast_1d(np.asarray(streams)))
+        if a.ndim != 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError("%s: expected a list of stream indices, got %s" % (name, np.shape(streams)))
+        return np.ascontiguousarray(a, np.int32)
+
+    def state_bytes(self):
+        """Bytes of one stream's state record."""
+        n = self._lib.b200s_stream_state_bytes(self._h)
+        self._ck(min(n, 0))
+        return n
+
+    def copy_streams(self, dst_streams, src_streams, src=None):
+        """Stream dst_streams[i] of this engine becomes a copy of stream src_streams[i] of `src` (default: this engine), as
+        the reference's copy assignment would make it.  Asynchronous on both engines' streams; swaps and forks work."""
+        src = self if src is None else src
+        if src._lib is not self._lib:
+            raise ValueError("copy_streams: both engines must come from the same library")
+        d, s = self._stream_list(dst_streams, "dst_streams"), self._stream_list(src_streams, "src_streams")
+        if d.size != s.size:
+            raise ValueError("copy_streams: %d destinations for %d sources" % (d.size, s.size))
+        ip = ctypes.POINTER(ctypes.c_int)
+        self._ck(self._lib.b200s_copy_streams(self._h, d.ctypes.data_as(ip), src._h, s.ctypes.data_as(ip), int(d.size)))
+
+    def export_streams(self, streams):
+        """The listed streams' state records: uint8 [n, state_bytes()]."""
+        s = self._stream_list(streams, "streams")
+        out = np.empty((s.size, self.state_bytes()), np.uint8)
+        self._ck(self._lib.b200s_export_streams(self._h, s.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), int(s.size), out.ctypes.data))
+        return out
+
+    def import_streams(self, streams, records):
+        """Load records of export_streams() (this configuration) into the listed slots."""
+        s = self._stream_list(streams, "streams")
+        r = np.ascontiguousarray(records, np.uint8)
+        if r.shape != (s.size, self.state_bytes()):
+            raise ValueError("import_streams: expected records of shape %s, got %s" % ((s.size, self.state_bytes()), r.shape))
+        self._ck(self._lib.b200s_import_streams(self._h, s.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), int(s.size), r.ctypes.data))
+
+    def clone(self):
+        """A new engine with this one's batch, device, seed, configuration, tuning, parameters and state of every stream."""
+        h = ctypes.c_void_p()
+        self._ck(self._lib.b200s_clone(self._h, ctypes.byref(h)))
+        c = BatchStretch.__new__(BatchStretch)
+        c._lib, c._h, c.batch = self._lib, h, self.batch
+        return c
 
     # ---- plumbing ----
     def set_stream(self, cuda_stream):

@@ -34,6 +34,7 @@
 #include "chain_ws.cuh"
 #include "chain_direct6.cuh"
 #include "chain_t.cuh"
+#include "state_copy.cuh"
 
 using namespace b200s;
 
@@ -138,6 +139,17 @@ struct b200s_engine {
 	size_t inCap = 0, outCap = 0, zeroCap = 0, tmpCap = 0;
 	short *dIn16 = 0, *dOut16 = 0; // 16-bit PCM staging of b200s_process_pcm16
 	size_t in16Cap = 0, out16Cap = 0;
+	// stream copies, export and import (DESIGN.md §3.12): packed records [xferCap][record bytes], the stream lists of the
+	// pack and the unpack (device [2][xferCap]; two pinned staging copies, rewritten once the upload issued from them two
+	// uploads ago has run), and the event by which another handle orders its side of a copy after this one's
+	char *dXfer = 0;
+	int *dXferIdx = 0;
+	int xferCap = 0, xferRecCap = 0; // streams the lists / the records have room for
+	int *pinIdx[2] = {0, 0};
+	cudaEvent_t evIdx[2] = {0, 0};
+	int idxSlot = 0;
+	cudaEvent_t evXfer = 0;
+	std::vector<float> hMapIn, hMapOut; // host copy of the frequency-map table: a stream that uses it may only go to an engine with the same table
 };
 
 #define CK(call)                                                                                   \
@@ -1349,6 +1361,242 @@ static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStri
 }
 
 // =================================================================================================
+// Stream state records (b200s_copy_streams / _export_streams / _import_streams / _clone, DESIGN.md §3.12)
+// =================================================================================================
+// The host-written head of a record: what import checks before anything is enqueued, and the host-held part of the
+// stream (its parameters and the engine-wide random-path flags it carries).  Native byte order.
+struct StreamRecordHeader {
+	char magic[8];     // "B200SREC"
+	uint32_t version;  // kRecordVersion
+	uint32_t bytes;    // record size
+	int32_t C, B, H, split, K;
+	uint32_t flags;    // kRecPrevRandom | kRecSeekRandom | kRecUsesTable
+	int32_t mapN;      // the frequency-map table the stream uses (kRecUsesTable): its points and fingerprint
+	uint64_t mapHash;
+	StreamParams params;
+};
+static_assert(sizeof(StreamRecordHeader) <= B200S_RECORD_HEADER, "record header");
+static const uint32_t kRecordVersion = 1;
+enum { kRecPrevRandom = 1, kRecSeekRandom = 2, kRecUsesTable = 4 };
+
+static StateRegions state_regions(const b200s_engine *e) {
+	const Cfg &g = e->cfg;
+	const size_t CK = (size_t)g.C * g.K;
+	const struct { void *p; size_t bytes; } a[B200S_STATE_REGIONS] = {
+		{e->dSched, sizeof(Sched)},
+		{e->dRng, sizeof(unsigned)},
+		{e->dStPitch, 2 * sizeof(float)},
+		{e->dHist[e->histCur], sizeof(float) * g.C * g.histLen},
+		{e->dPend, sizeof(float) * g.C * g.pendLen},
+		{e->dPendWp, sizeof(float) * g.C * g.pendLen},
+		{e->dStIn, sizeof(float2) * CK},
+		{e->dStPrev, sizeof(float2) * CK},
+		{e->dStOut, sizeof(float2) * CK},
+		{e->dStPredE, sizeof(float) * CK},
+	};
+	StateRegions t;
+	unsigned off = B200S_RECORD_HEADER;
+	for (int i = 0; i < B200S_STATE_REGIONS; ++i) {
+		t.r[i].base = (char *)a[i].p;
+		t.r[i].bytes = (unsigned)a[i].bytes;
+		t.r[i].off = off;
+		off += (unsigned)((a[i].bytes + 15) / 16 * 16);
+	}
+	t.recBytes = off;
+	return t;
+}
+static bool uses_table(const b200s_engine *e, const StreamParams &p) { return p.customMap && e->fmap.mapN > 0; }
+static bool same_table(const b200s_engine *a, const b200s_engine *b) {
+	const size_t n = a->hMapIn.size();
+	return a->fmap.mapN == b->fmap.mapN && b->hMapIn.size() == n && b->hMapOut.size() == n &&
+	       (n == 0 || (!memcmp(a->hMapIn.data(), b->hMapIn.data(), sizeof(float) * n) && !memcmp(a->hMapOut.data(), b->hMapOut.data(), sizeof(float) * n)));
+}
+static uint64_t table_hash(const b200s_engine *e) { // FNV-1a over the points
+	uint64_t h = 1469598103934665603ull;
+	auto mix = [&](const void *p, size_t n) {
+		for (size_t i = 0; i < n; ++i) h = (h ^ ((const unsigned char *)p)[i]) * 1099511628211ull;
+	};
+	const int32_t n = e->fmap.mapN;
+	mix(&n, sizeof(n));
+	mix(e->hMapIn.data(), sizeof(float) * e->hMapIn.size());
+	mix(e->hMapOut.data(), sizeof(float) * e->hMapOut.size());
+	return h;
+}
+static bool same_config(const Cfg &a, const Cfg &b) { return a.C == b.C && a.B == b.B && a.H == b.H && a.split == b.split; }
+static std::string cfg_text(const Cfg &g) {
+	return std::to_string(g.C) + " channels, block " + std::to_string(g.B) + ", interval " + std::to_string(g.H) + (g.split ? ", split" : "");
+}
+
+// a list of n stream indices, checked against [0, S) and (unique) for duplicates; the message names the first bad entry
+static bool check_streams(std::string &err, const char *fn, const char *what, const int *streams, int n, int S, bool unique) {
+	if (n > 0 && !streams) {
+		err = std::string(fn) + ": " + what + " must not be NULL";
+		return false;
+	}
+	std::vector<char> seen(unique ? (size_t)S : 0, 0);
+	for (int i = 0; i < n; ++i) {
+		const int s = streams[i];
+		if (s < 0 || s >= S) {
+			err = std::string(fn) + ": " + what + "[" + std::to_string(i) + "] = " + std::to_string(s) + " is outside [0, " + std::to_string(S) + ")";
+			return false;
+		}
+		if (unique && seen[s]++) {
+			err = std::string(fn) + ": " + what + "[" + std::to_string(i) + "]: stream " + std::to_string(s) + " is listed twice";
+			return false;
+		}
+	}
+	return true;
+}
+
+// Staging of copies / export / import for n streams (records only when `records`): grows, never shrinks.  Growing
+// synchronises the handle's stream first, which has also waited for every other handle's read of these records.
+static int ensure_xfer(b200s_engine *e, int n, bool records) {
+	int rc;
+	if (n > e->xferCap) {
+		CK(cudaStreamSynchronize(e->stream));
+		for (int k = 0; k < 2; ++k) {
+			host_free(e->pinIdx[k]);
+			e->pinIdx[k] = 0;
+			if (!host_alloc((void **)&e->pinIdx[k], sizeof(int) * 2 * (size_t)n)) {
+				e->err = "pinned host memory allocation failed";
+				return B200S_ECUDA;
+			}
+		}
+		if ((rc = dalloc(e, &e->dXferIdx, 2 * (size_t)n))) return rc;
+		e->xferCap = n;
+	}
+	if (records && n > e->xferRecCap) {
+		CK(cudaStreamSynchronize(e->stream));
+		if ((rc = dalloc(e, &e->dXfer, (size_t)n * state_regions(e).recBytes))) return rc;
+		e->xferRecCap = n;
+	}
+	return 0;
+}
+// the stream lists of this handle's next pack (first half of dXferIdx) and / or unpack (second half), on its stream
+static int upload_lists(b200s_engine *e, const int *pack, const int *unpack, int n) {
+	const int k = e->idxSlot ^= 1;
+	CK(cudaEventSynchronize(e->evIdx[k]));
+	int *h = e->pinIdx[k];
+	if (pack) {
+		memcpy(h, pack, sizeof(int) * n);
+		CK(cudaMemcpyAsync(e->dXferIdx, h, sizeof(int) * n, cudaMemcpyHostToDevice, e->stream));
+	}
+	if (unpack) {
+		memcpy(h + e->xferCap, unpack, sizeof(int) * n);
+		CK(cudaMemcpyAsync(e->dXferIdx + e->xferCap, h + e->xferCap, sizeof(int) * n, cudaMemcpyHostToDevice, e->stream));
+	}
+	CK(cudaEventRecord(e->evIdx[k], e->stream));
+	return 0;
+}
+static dim3 xfer_grid(const StateRegions &t, int n) {
+	const unsigned chunks = (t.recBytes - B200S_RECORD_HEADER) / 16;
+	return dim3((chunks + 255) / 256, (unsigned)std::min(n, 65535));
+}
+static int launch_pack(b200s_engine *e, int n) {
+	const StateRegions t = state_regions(e);
+	B200S_LAUNCH(k_pack_streams, xfer_grid(t, n), dim3(256), 0, e->stream, t, (const int *)e->dXferIdx, n, e->dXfer);
+	CKL();
+	return 0;
+}
+static int launch_unpack(b200s_engine *e, int n, const char *records) {
+	const StateRegions t = state_regions(e);
+	B200S_LAUNCH(k_unpack_streams, xfer_grid(t, n), dim3(256), 0, e->stream, t, (const int *)e->dXferIdx + e->xferCap, n, records);
+	CKL();
+	return 0;
+}
+// restores the caller's current device when a call that works on a handle's (or two handles') devices returns (the
+// CPU emulator of the tests has one device and no device query: nothing to restore there)
+struct DeviceGuard {
+	int prev = -1;
+	DeviceGuard() {
+#ifndef B200S_EMU
+		if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+#endif
+	}
+	~DeviceGuard() {
+		if (prev >= 0) cudaSetDevice(prev);
+	}
+};
+// packed records from one device to another, without peer access enabled (the emulator has one device: never called)
+static cudaError_t copy_records_peer(char *dst, int dstDevice, const char *src, int srcDevice, size_t bytes, cudaStream_t st) {
+#ifdef B200S_EMU
+	(void)dstDevice;
+	(void)srcDevice;
+	return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st);
+#else
+	return cudaMemcpyPeerAsync(dst, dstDevice, src, srcDevice, bytes, st);
+#endif
+}
+
+// Everything b200s_copy_streams refuses, checked before anything is enqueued; the message goes to both handles
+static int check_copy(b200s_engine *dst, const int *dstS, b200s_engine *src, const int *srcS, int n) {
+	const char *fn = "b200s_copy_streams";
+	std::string err;
+	if (n < 0) err = std::string(fn) + ": negative stream count";
+	else if (!src->configured || !dst->configured) err = std::string(fn) + ": " + (src->configured ? "destination" : "source") + " engine not configured";
+	else if (!same_config(src->cfg, dst->cfg))
+		err = std::string(fn) + ": configurations differ (source " + cfg_text(src->cfg) + "; destination " + cfg_text(dst->cfg) + ")";
+	else if (check_streams(err, fn, "src_streams", srcS, n, src->S, false) && check_streams(err, fn, "dst_streams", dstS, n, dst->S, true) && src != dst) {
+		const bool tables = same_table(src, dst);
+		for (int i = 0; i < n && !tables; ++i)
+			if (uses_table(src, src->hSprm[srcS[i]])) {
+				err = std::string(fn) + ": src_streams[" + std::to_string(i) + "]: stream " + std::to_string(srcS[i]) +
+				      " uses the source's frequency-map table, and the destination's table differs";
+				break;
+			}
+	}
+	if (err.empty()) return 0;
+	src->err = dst->err = err;
+	return B200S_EINVAL;
+}
+// b200s_copy_streams, arguments checked: one pack on the source's stream, the records across to the destination's device
+// when it is another, one unpack on the destination's stream; then the host-held part
+static int copy_impl(b200s_engine *dst, const int *dstS, b200s_engine *src, const int *srcS, int n) {
+	if (n == 0) return 0;
+	DeviceGuard guard;
+	const bool same = src == dst, peer = src->device != dst->device;
+	int rc;
+	{
+		b200s_engine *e = src;
+		CK(cudaSetDevice(src->device));
+		if ((rc = ensure_xfer(src, n, true))) return rc;
+		if ((rc = upload_lists(src, srcS, same ? dstS : nullptr, n))) return rc;
+		src->chainedGroups = 0; // (a chained host-buffer call's stream groups would not wait for the pack)
+		if ((rc = launch_pack(src, n))) return rc;
+		if (!same) CK(cudaEventRecord(src->evXfer, src->stream));
+	}
+	if (same) {
+		if ((rc = launch_unpack(dst, n, dst->dXfer))) return rc;
+	} else {
+		b200s_engine *e = dst;
+		CK(cudaSetDevice(dst->device));
+		if ((rc = ensure_xfer(dst, n, peer))) return rc;
+		if ((rc = upload_lists(dst, nullptr, dstS, n))) return rc;
+		CK(cudaStreamWaitEvent(dst->stream, src->evXfer, 0));
+		const size_t bytes = (size_t)n * state_regions(src).recBytes;
+		if (peer) CK(copy_records_peer(dst->dXfer, dst->device, src->dXfer, src->device, bytes, dst->stream));
+		if ((rc = launch_unpack(dst, n, peer ? dst->dXfer : src->dXfer))) return rc;
+		// the source's records are free again once the destination has read them
+		CK(cudaEventRecord(dst->evXfer, dst->stream));
+		e = src;
+		CK(cudaSetDevice(src->device));
+		CK(cudaStreamWaitEvent(src->stream, dst->evXfer, 0));
+	}
+	dst->chainedGroups = 0;
+	// parameters through the host table (read before any is written: swaps and forks), uploaded by the next call
+	std::vector<StreamParams> p((size_t)n);
+	for (int i = 0; i < n; ++i) {
+		p[i] = src->hSprm[srcS[i]];
+		if (!same && !uses_table(src, p[i])) p[i].customMap = 0;
+	}
+	for (int i = 0; i < n; ++i) dst->hSprm[dstS[i]] = p[i];
+	params_changed(dst);
+	dst->prevCallMayRandom = dst->prevCallMayRandom || src->prevCallMayRandom;
+	dst->seekMayRandom = dst->seekMayRandom || src->seekMayRandom;
+	return 0;
+}
+
+// =================================================================================================
 // extern "C" ABI
 // =================================================================================================
 extern "C" {
@@ -1399,6 +1647,8 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 	for (int k = 0; k < 2; ++k) {
 		bool ok = host_alloc((void **)&e->pinSprm[k], sizeof(StreamParams) * (size_t)batch) &&
 		          cudaEventCreateWithFlags(&e->evSprm[k], cudaEventDisableTiming) == cudaSuccess &&
+		          cudaEventCreateWithFlags(&e->evIdx[k], cudaEventDisableTiming) == cudaSuccess &&
+		          (k || cudaEventCreateWithFlags(&e->evXfer, cudaEventDisableTiming) == cudaSuccess) &&
 		          host_alloc((void **)&e->pinDesc[k], sizeof(CallDesc) * (size_t)batch);
 		for (int i = 0; i < b200s_engine::kMaxSub && ok; ++i) ok = cudaEventCreateWithFlags(&e->evDesc[k][i], cudaEventDisableTiming) == cudaSuccess;
 		if (!ok) {
@@ -1440,7 +1690,12 @@ void b200s_destroy(b200s_engine *e) {
 	dfree(e->dSeekEnd);
 	dfree(e->dSprm);
 	dfree(e->dDesc);
+	dfree(e->dXfer);
+	dfree(e->dXferIdx);
+	if (e->evXfer) cudaEventDestroy(e->evXfer);
 	for (int k = 0; k < 2; ++k) {
+		host_free(e->pinIdx[k]);
+		if (e->evIdx[k]) cudaEventDestroy(e->evIdx[k]);
 		host_free(e->pinSprm[k]);
 		if (e->evSprm[k]) cudaEventDestroy(e->evSprm[k]);
 		host_free(e->pinDesc[k]);
@@ -1626,6 +1881,8 @@ int b200s_set_freq_map_table(b200s_engine *e, const float *fin, const float *fou
 	dfree(e->dMapIn);
 	dfree(e->dMapOut);
 	e->fmap.mapN = 0;
+	e->hMapIn.assign(fin, fin + n);
+	e->hMapOut.assign(fout, fout + n);
 	for (StreamParams &p : e->hSprm) p.customMap = 1; // one table per engine, used by every stream until a transpose setter
 	params_changed(e);
 	if (n == 0) return 0;
@@ -1923,6 +2180,133 @@ int b200s_set_state(b200s_engine *e, int what, const float *src) {
 	CK(cudaStreamSynchronize(e->stream));
 	CK(cudaMemcpy(p, src, sizeof(float) * n * e->S, cudaMemcpyHostToDevice));
 	return 0;
+}
+
+// ---- stream state records ----
+int b200s_stream_state_bytes(const b200s_engine *e) {
+	if (!e || !e->configured) return B200S_EINVAL;
+	return (int)state_regions(e).recBytes;
+}
+int b200s_copy_streams(b200s_engine *dst, const int *dst_streams, b200s_engine *src, const int *src_streams, int n) {
+	if (!dst || !src) return B200S_EINVAL;
+	int rc;
+	if ((rc = check_copy(dst, dst_streams, src, src_streams, n))) return rc;
+	return copy_impl(dst, dst_streams, src, src_streams, n);
+}
+int b200s_export_streams(b200s_engine *e, const int *streams, int n, void *host_dst) {
+	NEED_CFG();
+	if (n < 0 || (n > 0 && !host_dst)) {
+		e->err = std::string("b200s_export_streams: ") + (n < 0 ? "negative stream count" : "host_dst must not be NULL");
+		return B200S_EINVAL;
+	}
+	if (!check_streams(e->err, "b200s_export_streams", "streams", streams, n, e->S, false)) return B200S_EINVAL;
+	if (n == 0) return 0;
+	DeviceGuard guard;
+	CK(cudaSetDevice(e->device));
+	int rc;
+	if ((rc = ensure_xfer(e, n, true))) return rc;
+	if ((rc = upload_lists(e, streams, nullptr, n))) return rc;
+	if ((rc = launch_pack(e, n))) return rc;
+	const size_t R = state_regions(e).recBytes;
+	CK(cudaMemcpyAsync(host_dst, e->dXfer, (size_t)n * R, cudaMemcpyDeviceToHost, e->stream));
+	CK(cudaStreamSynchronize(e->stream));
+	const uint64_t hash = table_hash(e);
+	for (int i = 0; i < n; ++i) {
+		StreamRecordHeader h;
+		memset(&h, 0, sizeof(h));
+		memcpy(h.magic, "B200SREC", 8);
+		h.version = kRecordVersion;
+		h.bytes = (uint32_t)R;
+		h.C = e->cfg.C; h.B = e->cfg.B; h.H = e->cfg.H; h.split = e->cfg.split; h.K = e->cfg.K;
+		h.params = e->hSprm[streams[i]];
+		h.flags = (e->prevCallMayRandom ? kRecPrevRandom : 0) | (e->seekMayRandom ? kRecSeekRandom : 0);
+		if (uses_table(e, h.params)) {
+			h.flags |= kRecUsesTable;
+			h.mapN = e->fmap.mapN;
+			h.mapHash = hash;
+		} else {
+			h.params.customMap = 0;
+		}
+		char *rec = (char *)host_dst + (size_t)i * R;
+		memset(rec, 0, B200S_RECORD_HEADER);
+		memcpy(rec, &h, sizeof(h));
+	}
+	return 0;
+}
+int b200s_import_streams(b200s_engine *e, const int *streams, int n, const void *host_src) {
+	NEED_CFG();
+	const char *fn = "b200s_import_streams";
+	if (n < 0 || (n > 0 && !host_src)) {
+		e->err = std::string(fn) + ": " + (n < 0 ? "negative stream count" : "host_src must not be NULL");
+		return B200S_EINVAL;
+	}
+	if (!check_streams(e->err, fn, "streams", streams, n, e->S, true)) return B200S_EINVAL;
+	const size_t R = state_regions(e).recBytes;
+	const uint64_t hash = table_hash(e);
+	std::vector<StreamRecordHeader> hs((size_t)n);
+	for (int i = 0; i < n; ++i) {
+		StreamRecordHeader &h = hs[i];
+		memcpy(&h, (const char *)host_src + (size_t)i * R, sizeof(h));
+		std::string why;
+		if (memcmp(h.magic, "B200SREC", 8)) why = "not a stream record";
+		else if (h.version != kRecordVersion) why = "record format " + std::to_string(h.version) + ", this library reads " + std::to_string(kRecordVersion);
+		else if (h.C != e->cfg.C || h.B != e->cfg.B || h.H != e->cfg.H || h.split != e->cfg.split || h.K != e->cfg.K || h.bytes != R)
+			why = "recorded with another configuration (" + std::to_string(h.C) + " channels, block " + std::to_string(h.B) + ", interval " +
+			      std::to_string(h.H) + (h.split ? ", split" : "") + "; this engine: " + cfg_text(e->cfg) + ")";
+		else if ((h.flags & kRecUsesTable) && (h.mapN != e->fmap.mapN || h.mapHash != hash))
+			why = "the stream uses a frequency-map table that differs from this engine's";
+		if (!why.empty()) {
+			e->err = std::string(fn) + ": record " + std::to_string(i) + ": " + why;
+			return B200S_EINVAL;
+		}
+	}
+	if (n == 0) return 0;
+	DeviceGuard guard;
+	CK(cudaSetDevice(e->device));
+	int rc;
+	if ((rc = ensure_xfer(e, n, true))) return rc;
+	if ((rc = upload_lists(e, nullptr, streams, n))) return rc;
+	CK(cudaMemcpyAsync(e->dXfer, host_src, (size_t)n * R, cudaMemcpyHostToDevice, e->stream));
+	e->chainedGroups = 0;
+	if ((rc = launch_unpack(e, n, e->dXfer))) return rc;
+	for (int i = 0; i < n; ++i) {
+		e->hSprm[streams[i]] = hs[i].params;
+		e->prevCallMayRandom = e->prevCallMayRandom || (hs[i].flags & kRecPrevRandom);
+		e->seekMayRandom = e->seekMayRandom || (hs[i].flags & kRecSeekRandom);
+	}
+	params_changed(e);
+	CK(cudaStreamSynchronize(e->stream));
+	return 0;
+}
+int b200s_clone(b200s_engine *src, b200s_engine **out) {
+	if (!src || !out) {
+		g_createError = "b200s_clone: bad arguments";
+		return B200S_EINVAL;
+	}
+	*out = 0;
+	b200s_engine *e = 0;
+	int rc;
+	if ((rc = b200s_create(src->S, src->seed, src->device, &e))) {
+		src->err = g_createError;
+		return rc;
+	}
+	e->chainV = src->chainV; e->fftV1 = src->fftV1; e->nHostParts = src->nHostParts; e->exactMath = src->exactMath;
+	e->stepMajor = src->stepMajor; e->dual = src->dual; e->nSub = src->nSub;
+	const int mapN = src->fmap.mapN;
+	if (mapN > 0 && (rc = b200s_set_freq_map_table(e, src->hMapIn.data(), src->hMapOut.data(), mapN))) goto fail;
+	e->hSprm = src->hSprm; // (setting the table turned it on for every stream)
+	params_changed(e);
+	if (src->configured) {
+		std::vector<int> all((size_t)src->S);
+		for (int s = 0; s < src->S; ++s) all[s] = s;
+		if ((rc = configure_impl(e, src->cfg.C, src->cfg.B, src->cfg.H, src->cfg.split)) || (rc = copy_impl(e, all.data(), src, all.data(), src->S))) goto fail;
+	}
+	*out = e;
+	return 0;
+fail:
+	src->err = g_createError = "b200s_clone: " + e->err;
+	b200s_destroy(e);
+	return rc;
 }
 
 } // extern "C"
