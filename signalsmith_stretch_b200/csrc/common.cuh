@@ -148,6 +148,7 @@ struct Ctx {
 	const StreamParams *sprm; // [S] per-stream parameters
 	// tables
 	const float *window, *winProd, *wpReset;
+	const float *wpDiv; // [H] windowProducts of a slot covered by a full H-spaced run of blocks, by phase (k_synth2)
 	const float2 *rot, *twiddle, *pretw;
 	const float4 *anaTab; // [K] {window[n+o], window[n+o-K], pretw[n].x, pretw[n].y}: one load per element in k_analyse2
 	float2 rot0, rotStep; // rot[b+1] = rot[b] * rotStep in float, the reference's own recurrence (:647-655)

@@ -95,7 +95,7 @@ struct b200s_engine {
 	std::vector<int> profKind;
 
 	// tables
-	float *dWindow = 0, *dWinProd = 0, *dWpReset = 0;
+	float *dWindow = 0, *dWinProd = 0, *dWpReset = 0, *dWpDiv = 0;
 	float2 *dRot = 0, *dTwiddle = 0, *dPretw = 0;
 	float4 *dAnaTab = 0;
 	float2 rot0, rotStep;
@@ -206,7 +206,7 @@ static void host_free(void *p) {
 }
 
 static void free_all(b200s_engine *e) {
-	dfree(e->dWindow); dfree(e->dWinProd); dfree(e->dWpReset); dfree(e->dRot); dfree(e->dTwiddle); dfree(e->dPretw); dfree(e->dAnaTab);
+	dfree(e->dWindow); dfree(e->dWinProd); dfree(e->dWpReset); dfree(e->dWpDiv); dfree(e->dRot); dfree(e->dTwiddle); dfree(e->dPretw); dfree(e->dAnaTab);
 	dfree(e->dSched); dfree(e->dHist[0]); dfree(e->dHist[1]); dfree(e->dPend); dfree(e->dPendWp);
 	dfree(e->dStIn); dfree(e->dStPrev); dfree(e->dStOut); dfree(e->dStPredE); dfree(e->dStIl);
 	dfree(e->dFrames); dfree(e->dCall); dfree(e->dJobs); dfree(e->dSpec); dfree(e->dY); dfree(e->dPI); dfree(e->dFT); dfree(e->dT1); dfree(e->dT2); dfree(e->dE); dfree(e->dS); dfree(e->dM); dfree(e->dT1u); dfree(e->dT2u); dfree(e->dRngPow); dfree(e->dStPitch);
@@ -226,7 +226,7 @@ static Ctx make_ctx(b200s_engine *e) {
 	x.fmap.mapIn = e->dMapIn;
 	x.fmap.mapOut = e->dMapOut;
 	x.sprm = e->dSprm;
-	x.window = e->dWindow; x.winProd = e->dWinProd; x.wpReset = e->dWpReset;
+	x.window = e->dWindow; x.winProd = e->dWinProd; x.wpReset = e->dWpReset; x.wpDiv = e->dWpDiv;
 	x.rot = e->dRot; x.twiddle = e->dTwiddle; x.pretw = e->dPretw; x.anaTab = e->dAnaTab;
 	x.rot0 = e->rot0; x.rotStep = e->rotStep;
 	x.one = 1.0f;
@@ -327,7 +327,28 @@ static ChainKernel analyse2_kernel(const Cfg &g, bool mixed = false) {
 #endif
 	return g.K == 3072 ? k_analyse2<3072> : k_analyse2<2560>;
 }
-static ChainKernel synth2_kernel(const Cfg &g) { return g.K == 3072 ? k_synth2<3072> : k_synth2<2560>; }
+#ifdef B200S_SYNTH_PROBES // profiling builds only: ablations of k_synth2<3072> (wrong results), B200S_SYNTH_PROBE=1..4
+static int synth_probe() {
+	static int probe = -1;
+	if (probe < 0) {
+		const char *pv = getenv("B200S_SYNTH_PROBE");
+		probe = pv ? atoi(pv) : 0;
+	}
+	return probe;
+}
+#endif
+static ChainKernel synth2_kernel(const Cfg &g) {
+#ifdef B200S_SYNTH_PROBES
+	if (g.K == 3072) switch (synth_probe()) {
+		case 1: return k_synth2_probe<3072, 1>;
+		case 2: return k_synth2_probe<3072, 2>;
+		case 3: return k_synth2_probe<3072, 3>;
+		case 4: return k_synth2_probe<3072, 4>;
+		default: break;
+		}
+#endif
+	return g.K == 3072 ? k_synth2<3072> : k_synth2<2560>;
+}
 #ifdef B200S_KEEP_OLD_KERNELS
 static ChainKernel synth_kernel(const Cfg &g) { return g.K == 3072 ? k_synth<3072> : g.K == 2560 ? k_synth<2560> : k_synth<0>; }
 #else
@@ -577,7 +598,7 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 	e->cfg = g;
 
 	// ---- tables.  Window: Kaiser, the dependency's bandwidth heuristic, forced perfect reconstruction (App. B)
-	std::vector<float> window(g.B), winProd(g.B), wpReset(g.pendLen);
+	std::vector<float> window(g.B), winProd(g.B), wpReset(g.pendLen), wpDiv(g.H);
 	{
 		double bw = double(g.B) / double(g.H);
 		bw += 8 / ((bw + 3) * (bw + 3)) + 0.25 * std::max(3 - bw, 0.0);
@@ -608,6 +629,13 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 				wpReset[i] = B200S_ALMOST_ZERO;
 			}
 		}
+		// windowProducts of a slot at phase j that every block of a run H apart has reached: the ceil((B - j) / H) blocks
+		// that cover it, added to the cleared slot oldest first, as the overlap-add ring does (:397-399)
+		for (int j = 0; j < g.H; ++j) {
+			float sum = B200S_ALMOST_ZERO;
+			for (int k = (g.B - j + g.H - 1) / g.H - 1; k >= 0; --k) sum = sum + winProd[j + k * g.H];
+			wpDiv[j] = sum;
+		}
 	}
 	std::vector<float2> rot(g.K), tw(g.K), pre(g.K);
 	{ // :647-655, the reference's own float recurrence (its rounding is part of the result)
@@ -630,12 +658,14 @@ static int configure_impl(b200s_engine *e, int channels, int block, int interval
 	if ((rc = dalloc(e, &e->dWindow, g.B))) return rc;
 	if ((rc = dalloc(e, &e->dWinProd, g.B))) return rc;
 	if ((rc = dalloc(e, &e->dWpReset, g.pendLen))) return rc;
+	if ((rc = dalloc(e, &e->dWpDiv, g.H))) return rc;
 	if ((rc = dalloc(e, &e->dRot, g.K))) return rc;
 	if ((rc = dalloc(e, &e->dTwiddle, g.K))) return rc;
 	if ((rc = dalloc(e, &e->dPretw, g.K))) return rc;
 	CK(cudaMemcpy(e->dWindow, window.data(), sizeof(float) * g.B, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(e->dWinProd, winProd.data(), sizeof(float) * g.B, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(e->dWpReset, wpReset.data(), sizeof(float) * g.pendLen, cudaMemcpyHostToDevice));
+	CK(cudaMemcpy(e->dWpDiv, wpDiv.data(), sizeof(float) * g.H, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(e->dRot, rot.data(), sizeof(float2) * g.K, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(e->dTwiddle, tw.data(), sizeof(float2) * g.K, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(e->dPretw, pre.data(), sizeof(float2) * g.K, cudaMemcpyHostToDevice));

@@ -304,17 +304,20 @@ __global__ void __launch_bounds__(256, 2) k_analyse2_mixed(Ctx x) { analyse2_bod
 // ---------------------------------------------------------------------------------------------
 // k_synth2: grid (C, S), 256 threads, one CTA per stream-channel; blocks of the call two at a time.
 // dyn smem: PairGeo::LEN float4 (FFT pair; between two FFTs it holds the next pair's two spectra, staged by a bulk
-// copy) + pendLen floats (pending ring) + pendLen floats (windowProducts ring; kept per channel so that no two CTAs
-// share writable state).
+// copy) + pendLen floats (pending ring).  The windowProducts divisor is not carried in a ring: it depends on the block
+// schedule only, and each emitted sample computes its own (wp_at).
+// PROBE (profiling builds, -DB200S_SYNTH_PROBES; wrong results on purpose) removes one part of the kernel to measure what
+// its time goes with: 1 the windowProducts divisor (the samples are emitted undivided), 2 every ring update of the overlap-add,
+// 3 the wait for the staged spectra (moved to just before the next copies are issued), 4 the inverse FFT's passes 2-3.
 // ---------------------------------------------------------------------------------------------
-template <int KT>
-__global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
+template <int KT, int PROBE>
+__device__ __forceinline__ void synth2_body(const Ctx &x) {
 	using G = PairGeo<KT>;
 	static_assert(2 * KT * sizeof(float2) <= G::LEN * sizeof(float4), "the two spectra of a pair fit the FFT buffer");
 	const Cfg &g = x.cfg;
 	B200S_DYN_SHARED
 	float4 *buf = (float4 *)dyn_smem;
-	float *pend = (float *)(buf + G::LEN), *wp = pend + g.pendLen;
+	float *pend = (float *)(buf + G::LEN);
 	const int c = blockIdx.x, s = x.sBase + blockIdx.y, tid = threadIdx.x;
 	const Call cl = x.call[s];
 	float *out = x.out + (size_t)s * x.outStreamStride + (size_t)c * x.outChanStride;
@@ -347,12 +350,41 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 		}
 	};
 	if (cl.nFrames > 0) stage_pair(0);
-	for (int i = tid; i < P; i += 256) {
-		pend[i] = gp[i];
-		wp[i] = gw[i];
-	}
+	for (int i = tid; i < P; i += 256) pend[i] = gp[i];
 	__syncthreads();
 	int head = 0, emitted = 0;
+	// windowProducts (:397-399, :408-414) of output sample T of the call (T = emitted + ring offset): the carried value
+	// gw[T] (T < P; slots beyond were cleared to ALMOST_ZERO when emitted), plus winProd[u - f*H] of every block f of the call
+	// that covers it, in block order, u = T - addOff - t0.  k_plan triggers the blocks of a call exactly H apart from t0
+	// (samplesSinceLast restarts at 0 on a trigger, :281-286), so wherever T >= P and the covering blocks are the full
+	// H-spaced run (B - H <= u < nFrames*H), the sum is the table entry wpDiv[u mod H], accumulated in the same order.
+	// The other samples -- the first ones of a call and the ring's tail at its end -- add the terms one by one.
+	const int uOff = addOff + (cl.nFrames > 0 ? frames[0].t : 0);
+	auto wp_at = [&](int T) -> float {
+		const int u = T - uOff, H = g.H, nF = __ldg(&x.call[s].nFrames);
+		if (T >= P && u >= B - H && u < nF * H) return __ldg(x.wpDiv + u % H);
+		float w = T < P ? gw[T] : B200S_ALMOST_ZERO;
+		if (u >= 0)
+			for (int f = (u >= B ? (u - B) / H + 1 : 0), fHi = min(u / H, nF - 1); f <= fHi; ++f) w = fadd(w, __ldg(x.winProd + u - f * H));
+		return w;
+	};
+	// samples T .. T+3: one index computation for the four table entries when all four are in the full run
+	auto wp_at4 = [&](int T) -> float4 {
+		const int u = T - uOff, H = g.H, nF = __ldg(&x.call[s].nFrames);
+		if (T >= P && u >= B - H && u + 3 < nF * H) {
+			int j = u % H;
+			float4 w;
+			w.x = __ldg(x.wpDiv + j);
+			if (++j == H) j = 0;
+			w.y = __ldg(x.wpDiv + j);
+			if (++j == H) j = 0;
+			w.z = __ldg(x.wpDiv + j);
+			if (++j == H) j = 0;
+			w.w = __ldg(x.wpDiv + j);
+			return w;
+		}
+		return make_float4(wp_at(T), wp_at(T + 1), wp_at(T + 2), wp_at(T + 3));
+	};
 	// emit n samples from the ring head, zero them behind (:408-414)
 	// VECTOR form of the ring loops: when the ring head, the counts and the output row are multiples of four floats
 	// (the presets at 48 kHz with chunks that are multiples of four), four consecutive ring slots are one 16-byte
@@ -363,10 +395,14 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 			for (int i = 4 * tid; i < n; i += 1024) {
 				int p = head + i;
 				if (p >= P) p -= P;
-				const float4 a = *(float4 *)(pend + p), w = *(float4 *)(wp + p);
-				st_stream4(out + emitted + i, make_float4(fdiv(a.x, w.x), fdiv(a.y, w.y), fdiv(a.z, w.z), fdiv(a.w, w.w)));
+				const float4 a = *(float4 *)(pend + p);
+				if constexpr (PROBE == 1) {
+					st_stream4(out + emitted + i, a);
+				} else {
+					const float4 w = wp_at4(emitted + i);
+					st_stream4(out + emitted + i, make_float4(fdiv(a.x, w.x), fdiv(a.y, w.y), fdiv(a.z, w.z), fdiv(a.w, w.w)));
+				}
 				*(float4 *)(pend + p) = make_float4(0.f, 0.f, 0.f, 0.f);
-				*(float4 *)(wp + p) = make_float4(B200S_ALMOST_ZERO, B200S_ALMOST_ZERO, B200S_ALMOST_ZERO, B200S_ALMOST_ZERO);
 			}
 			head = (head + n) % P;
 			emitted += n;
@@ -377,9 +413,8 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 			if (i < P) {
 				int p = head + i;
 				if (p >= P) p -= P;
-				v = fdiv(pend[p], wp[p]);
+				v = PROBE == 1 ? pend[p] : fdiv(pend[p], wp_at(emitted + i));
 				pend[p] = 0.f;
-				wp[p] = B200S_ALMOST_ZERO;
 			}
 			st_stream(out + emitted + i, v);
 		}
@@ -391,12 +426,16 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 	// one owner, so the overlap-add goes from registers straight into the ring, one writing thread per slot.
 	// block A (hi = false) or B (hi = true) into the ring (:397-399): sample i lands in slot head + addOff + i
 	auto add_block = [&](const f2 (&yRe)[G::R3], const f2 (&yIm)[G::R3], bool hi) {
-		const float *winProd = x.winProd;
 		auto add = [&](int i, f2 y) {
 			int p = head + addOff + i;
 			if (p >= P) p -= P;
+			if constexpr (PROBE == 2) {
+#ifndef B200S_EMU
+				asm volatile("" ::"f"(hi ? f2_hi(y) : f2_lo(y)), "r"(p));
+#endif
+				return;
+			}
 			pend[p] = fadd(pend[p], hi ? f2_hi(y) : f2_lo(y));
-			wp[p] = fadd(wp[p], __ldg(winProd + i));
 		};
 		static_for<G::R3>([&](auto qc) {
 			constexpr int q3 = decltype(qc)::value;
@@ -424,8 +463,10 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 		// samples emitted between the two blocks; without a second block nothing is emitted between them
 		const int gap = hasB ? frames[f + 1].t - tA : 0;
 		emit(tA - emitted); // while the spectra are on their way
-		mbar_wait(&stageBar, stagePar);
-		stagePar ^= 1u;
+		if constexpr (PROBE != 3) {
+			mbar_wait(&stageBar, stagePar);
+			stagePar ^= 1u;
+		}
 		const float2 *sA = stY, *sB = hasB ? stY + KT : stY;
 #ifdef B200S_EMU_EXACT_FFT // test builds only: the oracle's double FFT, results handed over in the registers of the real path
 		{
@@ -475,7 +516,11 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 			// 2*Re(z[i-o] * conj(pre[i-o])) for i >= o and 2*Im(z[i-o+K] * conj(pre[i-o+K])) for i < o,
 			// so z[n2] yields sample n2+o (if < B) from its real part and sample n2+o-K (if >= 0) from its imaginary part
 			c2 z[G::R3];
-			pair_dif_pass23<KT>(buf, tw_bases(), tid, z); // (uses tw.b only)
+			if constexpr (PROBE == 4) {
+				static_for<G::R3>([&](auto qc) { z[decltype(qc)::value] = c2{f2_make((float)tid, 0.f), f2_make(0.f, (float)decltype(qc)::value)}; });
+			} else {
+				pair_dif_pass23<KT>(buf, tw_bases(), tid, z); // (uses tw.b only)
+			}
 			static_for<G::R3>([&](auto qc) {
 				constexpr int q3 = decltype(qc)::value;
 				const int n2 = (tid & 15) + 16 * (tid >> 4) + 256 * q3;
@@ -488,6 +533,10 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 		}
 #endif
 		__syncthreads(); // every read of buf has ended: the next pair's spectra may land there
+		if constexpr (PROBE == 3) {
+			mbar_wait(&stageBar, stagePar);
+			stagePar ^= 1u;
+		}
 		if (f + 2 < cl.nFrames) stage_pair(f + 2);
 		// ---- overlap-add, per ring slot in the reference's order: block A's sample, the emission of the samples
 		//      between the two blocks, then block B's sample (relative to the head after the emission)
@@ -509,13 +558,25 @@ __global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) {
 		for (int i = nOut + tid; i < x.outTail; i += 256) st_stream(out + i, 0.f); // (per-stream calls: the row's zero tail)
 	}
 	__syncthreads();
+	// the windowProducts the ring would carry into the next call, slot i for output sample emitted + i: gathered in the
+	// (now idle) FFT buffer before any is stored, since in a short call they read the carried values they replace
+	// (P <= B + H <= 2B < 2N floats: the buffer holds 4K)
+	float *wpNext = (float *)buf;
+	for (int i = tid; i < P; i += 256) wpNext[i] = wp_at(emitted + i);
+	__syncthreads();
 	for (int i = tid; i < P; i += 256) {
 		int p = head + i;
 		if (p >= P) p -= P;
 		gp[i] = pend[p];
-		gw[i] = wp[p];
+		gw[i] = wpNext[i];
 	}
 }
+template <int KT>
+__global__ void __launch_bounds__(256, 2) k_synth2(Ctx x) { synth2_body<KT, 0>(x); }
+#ifdef B200S_SYNTH_PROBES
+template <int KT, int PROBE>
+__global__ void __launch_bounds__(256, 2) k_synth2_probe(Ctx x) { synth2_body<KT, PROBE>(x); }
+#endif
 
 static inline size_t smem_analyse2(const Cfg &g) {
 	const int len = g.K == 3072 ? PairGeo<3072>::LEN : PairGeo<2560>::LEN;
@@ -523,7 +584,7 @@ static inline size_t smem_analyse2(const Cfg &g) {
 }
 static inline size_t smem_synth2(const Cfg &g) {
 	const int len = g.K == 3072 ? PairGeo<3072>::LEN : PairGeo<2560>::LEN;
-	return sizeof(float4) * len + sizeof(float) * 2 * g.pendLen;
+	return sizeof(float4) * len + sizeof(float) * g.pendLen;
 }
 
 } // namespace b200s
