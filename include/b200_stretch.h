@@ -105,9 +105,22 @@ int b200s_set_formant_base_per_stream(b200s_engine *e, const float *base_freqs);
  * "We can't do setFreqMap()", main.cpp:67).  The C++ facade tabulates the callable and passes a
  * monotone piecewise-linear map here: `n` points, freq_in[i] -> freq_out[i] (both as multiples
  * of the sample rate, freq_in ascending); linear extrapolation outside.  n == 0 clears it.
- * One table per engine: it applies to every stream, until a transpose setter (broadcast or per stream) turns it off
- * for every stream, as setTransposeFactor clears the reference's custom map. */
+ * The engine's table: it applies to every stream, replacing any table a stream had of its own, until a transpose setter
+ * (broadcast or per stream) turns it off for every stream it writes, as setTransposeFactor clears the reference's custom
+ * map.  May synchronise the handle's stream. */
 int b200s_set_freq_map_table(b200s_engine *e, const float *freq_in, const float *freq_out, int n);
+/* Every stream its own map: a server whose users each have their own pitch mapping (a harmoniser that snaps each user to
+ * that user's key) runs them in one batch.  Stream streams[i] gets its own table of n_points[i] points; the tables lie one
+ * after another in freq_in / freq_out (sum(n_points) floats each), with the same contract as b200s_set_freq_map_table.
+ * n_points[i] == 0: the stream has no custom map (the reference's customFreqMap = nullptr).  Streams that are not listed
+ * keep what they have; a later b200s_set_freq_map_table replaces every stream's table, and a transpose setter clears the
+ * map of every stream it writes.  Stream s is bit-identical to a one-stream engine given its table through
+ * b200s_set_freq_map_table.  Tables are kept once per distinct content (1024 streams that share 16 maps hold 16 tables).
+ * B200S_EINVAL before anything changes, b200s_last_error() naming the first bad entry: a NULL array with n > 0 (freq_in /
+ * freq_out: with sum(n_points) > 0), n < 0, a stream outside [0, batch) or listed twice, n_points[i] < 0.  May
+ * synchronise the handle's stream. */
+int b200s_set_freq_map_table_per_stream(b200s_engine *e, const int *streams, int n, const int *n_points,
+                                        const float *freq_in, const float *freq_out);
 
 /* ---- the hot path (:139-165 seek, :172-204 outputSeek, :209-423 process, :426-464 flush, :467-491 exact) ----
  * Host-buffer variants: `in`/`out` are host pointers, planar [batch][channels][samples]; the call
@@ -202,9 +215,11 @@ int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *d_
  *   - src == dst is allowed; src and dst may be different handles on the same or on different devices.  Both must have
  *     the same configuration (channels, block, interval, split); batch, seed and tuning keys may differ (exact math,
  *     key 3, included: the copy continues in the destination's arithmetic).
- *   - The frequency-map table is one per engine.  Within one engine a stream's use of it is copied as it is; a stream
- *     that uses it (set by b200s_set_freq_map_table with n > 0 and not cleared since) may only go to another engine whose
- *     table is bit-identical.  A stream that does not use it arrives not using the destination's.
+ *   - Frequency maps.  Within one engine a stream's table is copied as it is, without an upload.  A stream that uses the
+ *     engine's table (set by b200s_set_freq_map_table with n > 0 and not cleared since) may only go to another engine whose
+ *     table is bit-identical.  A stream with its own table (b200s_set_freq_map_table_per_stream) takes it along to the
+ *     other engine: the upload is ordered with the copy on the destination's stream, and only growing the destination's
+ *     table storage synchronises it.  A stream without a map arrives without one.
  *   - The parameters copied are the source's current ones (a setter called just before is included).  Whether the next
  *     call may need the random path (stretch beyond 2x, a slow seek) travels with the stream.
  *   - Ordering: the call acts as if it ran at its place in both handles' stream orders.  It enqueues without a host
@@ -213,12 +228,15 @@ int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *d_
  * b200s_export_streams writes n records of b200s_stream_state_bytes(e) bytes to host memory (synchronous);
  * b200s_import_streams reads them into the listed slots (synchronous).  A record starts with a header (magic, format
  * version, configuration, the stream's parameters and a fingerprint of the map table it uses); import checks every
- * header against the engine before anything is enqueued.  Records are in the host's byte order.
- * b200s_clone: a new handle with the same batch, device, seed, configuration, tuning keys, parameters, map table and
+ * header against the engine before anything is enqueued.  Records are in the host's byte order.  A record does not carry
+ * the map table itself: a stream that uses the engine's table imports into an engine with the same table, and a stream
+ * with its own table only into a slot that already holds a bit-identical table (its own or the engine's), which the
+ * caller that checkpointed the stream sets first.
+ * b200s_clone: a new handle with the same batch, device, seed, configuration, tuning keys, parameters, map tables and
  * state of every stream (an unconfigured source gives an unconfigured clone).  The copy members of the C++ facade.
  * B200S_EINVAL before anything is enqueued, b200s_last_error() naming the first offending entry (for a copy on both
  * handles): NULL arrays with n > 0, n < 0, an index outside [0, batch), duplicate destinations, an unconfigured engine,
- * a configuration mismatch, a bad record header, a map-table mismatch.
+ * a configuration mismatch, a bad record header (unknown flags included), a map-table mismatch.
  * Copies and imports stage through device buffers that grow on first use (b200s_device_allocations counts them); a
  * later call with at most as many streams allocates nothing. */
 int b200s_stream_state_bytes(const b200s_engine *e); /* bytes of one stream's record; B200S_EINVAL if not configured */

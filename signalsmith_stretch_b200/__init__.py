@@ -27,7 +27,7 @@ ABI_SYMBOLS = [
     "b200s_output_latency", "b200s_split_computation", "b200s_seek_length", "b200s_output_seek_length",
     "b200s_fft_samples", "b200s_bands",
     "b200s_set_transpose_factor", "b200s_set_transpose_semitones", "b200s_set_formant_factor",
-    "b200s_set_formant_semitones", "b200s_set_formant_base", "b200s_set_freq_map_table",
+    "b200s_set_formant_semitones", "b200s_set_formant_base", "b200s_set_freq_map_table", "b200s_set_freq_map_table_per_stream",
     "b200s_set_transpose_factor_per_stream", "b200s_set_transpose_semitones_per_stream", "b200s_set_formant_factor_per_stream",
     "b200s_set_formant_semitones_per_stream", "b200s_set_formant_base_per_stream",
     "b200s_seek", "b200s_seek_rates", "b200s_live_seek", "b200s_output_seek", "b200s_process", "b200s_process_async", "b200s_process_pcm16", "b200s_flush", "b200s_exact",
@@ -93,6 +93,7 @@ def _bind(lib):
         "b200s_set_transpose_factor": (ci, [vp, cf, cf]), "b200s_set_transpose_semitones": (ci, [vp, cf, cf]),
         "b200s_set_formant_factor": (ci, [vp, cf, ci]), "b200s_set_formant_semitones": (ci, [vp, cf, ci]),
         "b200s_set_formant_base": (ci, [vp, cf]), "b200s_set_freq_map_table": (ci, [vp, fp, fp, ci]),
+        "b200s_set_freq_map_table_per_stream": (ci, [vp, ip, ci, ip, fp, fp]),
         "b200s_set_transpose_factor_per_stream": (ci, [vp, fp, fp]), "b200s_set_transpose_semitones_per_stream": (ci, [vp, fp, fp]),
         "b200s_set_formant_factor_per_stream": (ci, [vp, fp, ip]), "b200s_set_formant_semitones_per_stream": (ci, [vp, fp, ip]),
         "b200s_set_formant_base_per_stream": (ci, [vp, fp]),
@@ -271,22 +272,49 @@ class BatchStretch:
         else:
             self._ck(self._lib.b200s_set_formant_base_per_stream(self._h, a[0]))
 
-    def setFreqMap(self, inputToOutput, points=2049):
-        """setFreqMap(std::function) (:120): the callable is tabulated on [0, 0.5] (piecewise linear)."""
-        if inputToOutput is None:
-            self._ck(self._lib.b200s_set_freq_map_table(self._h, None, None, 0))
-            return
+    @staticmethod
+    def _tabulate(fn, points):
         fin = np.linspace(0.0, 0.5, points).astype(np.float32)
-        fout = np.array([inputToOutput(float(f)) for f in fin], np.float32)
-        fp = ctypes.POINTER(ctypes.c_float)
-        self._ck(self._lib.b200s_set_freq_map_table(self._h, fin.ctypes.data_as(fp), fout.ctypes.data_as(fp), points))
+        return fin, np.array([fn(float(f)) for f in fin], np.float32)
 
-    def setFreqMapTable(self, fin, fout):
-        """The piecewise-linear map itself (b200s_set_freq_map_table): break points fin (ascending) -> fout."""
-        fin = np.ascontiguousarray(fin, np.float32)
-        fout = np.ascontiguousarray(fout, np.float32)
+    def setFreqMap(self, inputToOutput, points=2049, streams=None):
+        """setFreqMap(std::function) (:120): the callable is tabulated on [0, 0.5] (piecewise linear).  With `streams`
+        (a list of stream indices), or a list of callables (one per listed stream, or per stream of the batch; None = no
+        map), the listed streams get their own maps and the others keep theirs."""
+        if streams is None and not isinstance(inputToOutput, (list, tuple)):
+            if inputToOutput is None:
+                self._ck(self._lib.b200s_set_freq_map_table(self._h, None, None, 0))
+                return
+            self.setFreqMapTable(*self._tabulate(inputToOutput, points))
+            return
+        fns = inputToOutput if isinstance(inputToOutput, (list, tuple)) else [inputToOutput] * len(streams)
+        self.setFreqMapTable([None if f is None else self._tabulate(f, points) for f in fns], streams=streams)
+
+    def setFreqMapTable(self, fin, fout=None, streams=None):
+        """The piecewise-linear map itself (b200s_set_freq_map_table): break points fin (ascending) -> fout.  Per stream
+        (b200s_set_freq_map_table_per_stream): `streams` lists the streams that get the table (fin, fout), or fin is a
+        list of (fin, fout) pairs, one per listed stream (or per stream of the batch when `streams` is None; None = no
+        map).  Streams that are not listed keep their maps."""
         fp = ctypes.POINTER(ctypes.c_float)
-        self._ck(self._lib.b200s_set_freq_map_table(self._h, fin.ctypes.data_as(fp), fout.ctypes.data_as(fp), len(fin)))
+        if streams is None and fout is not None:
+            fin = np.ascontiguousarray(fin, np.float32)
+            fout = np.ascontiguousarray(fout, np.float32)
+            self._ck(self._lib.b200s_set_freq_map_table(self._h, fin.ctypes.data_as(fp), fout.ctypes.data_as(fp), len(fin)))
+            return
+        tables = list(fin) if fout is None else [(fin, fout)] * len(streams)
+        streams = np.ascontiguousarray(range(self.batch) if streams is None else streams, np.int32)
+        if len(tables) != len(streams):
+            raise ValueError("%d tables for %d streams" % (len(tables), len(streams)))
+        tables = [(np.zeros(0, np.float32),) * 2 if t is None else (np.asarray(t[0], np.float32), np.asarray(t[1], np.float32)) for t in tables]
+        for a, b in tables:
+            if a.shape != b.shape or a.ndim != 1:
+                raise ValueError("freq_in and freq_out must be 1-D and of one length, got %s and %s" % (a.shape, b.shape))
+        points = np.array([len(a) for a, _ in tables], np.int32)
+        ain = np.ascontiguousarray(np.concatenate([a for a, _ in tables]) if tables else np.zeros(0), np.float32)
+        aout = np.ascontiguousarray(np.concatenate([b for _, b in tables]) if tables else np.zeros(0), np.float32)
+        ip = ctypes.POINTER(ctypes.c_int)
+        self._ck(self._lib.b200s_set_freq_map_table_per_stream(self._h, streams.ctypes.data_as(ip), len(streams), points.ctypes.data_as(ip),
+                                                               ain.ctypes.data_as(fp), aout.ctypes.data_as(fp)))
 
     # ---- the hot path ----
     def _shape(self, n):

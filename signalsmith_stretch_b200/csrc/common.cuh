@@ -56,7 +56,7 @@ struct Cfg {
 };
 
 // user parameters (:107-135) of one stream in the form map_freq / inv_map_formant take: built by stream_params from the
-// stream's entry of Ctx::sprm and the engine's frequency map table Ctx::fmap
+// stream's entry of Ctx::sprm and its table in the frequency-map pool Ctx::maps
 struct Params {
 	float freqMultiplier, freqTonalityLimit;
 	float formantMultiplier, invFormantMultiplier, formantBaseFreq;
@@ -65,21 +65,22 @@ struct Params {
 	const float *mapIn, *mapOut;
 };
 
-// the custom frequency map table (setFreqMap, :120): one per engine
-struct FreqMap {
-	int mapN; // >0: piecewise-linear map of mapN points
-	const float *mapIn, *mapOut;
-};
-
-// the parameters of one stream (b200s_set_*_per_stream; the broadcast setters write every entry)
-struct StreamParams {
+// what the setters write for one stream (b200s_set_*_per_stream; the broadcast setters write every entry), and what a
+// stream record carries
+struct StreamSettings {
 	float freqMultiplier, freqTonalityLimit;
 	float formantMultiplier, invFormantMultiplier, formantBaseFreq;
 	int formantCompensation;
-	int customMap; // the stream uses the engine's frequency map table (set by b200s_set_freq_map_table, cleared by a transpose setter)
+	int customMap; // the stream has a custom frequency map (setFreqMap, :120; cleared by a transpose setter): kMapEngine, kMapOwn
+};
+enum { kMapNone = 0, kMapEngine = 1, kMapOwn = 2 }; // StreamSettings::customMap: no table, the engine's table, its own table
+// the parameters of one stream (Ctx::sprm): its settings and the descriptor of its frequency-map table, which lies at
+// mapOff floats into the engine's pool (mapN inputs, then mapN outputs).  mapN is 0 when customMap is kMapNone.
+struct StreamParams : StreamSettings {
+	int mapOff, mapN;
 };
 // which path a stream's parameters need: frequency map (:300) and formant processing (:310); neither = pure time-stretch
-__host__ __device__ __forceinline__ bool stream_mapped(const StreamParams &p, int mapN) { return (p.customMap && mapN > 0) || p.freqMultiplier != 1.0f; }
+__host__ __device__ __forceinline__ bool stream_mapped(const StreamParams &p) { return p.mapN > 0 || p.freqMultiplier != 1.0f; }
 __host__ __device__ __forceinline__ bool stream_formants(const StreamParams &p, bool mapped) { return p.formantMultiplier != 1.0f || (p.formantCompensation && mapped); }
 
 // per-stream block scheduler state (:494-529)
@@ -144,7 +145,7 @@ struct Job {
 // everything a kernel needs, passed by value
 struct Ctx {
 	Cfg cfg;
-	FreqMap fmap;
+	const float *maps;        // the frequency-map pool: every table a stream uses (StreamParams::mapOff / mapN)
 	const StreamParams *sprm; // [S] per-stream parameters
 	// tables
 	const float *window, *winProd, *wpReset;

@@ -21,7 +21,9 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
+#include <climits>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/b200_stretch.h"
@@ -40,12 +42,44 @@ using namespace b200s;
 
 static std::string g_createError;
 
+// one frequency-map table (setFreqMap, :120) of the engine's pool: n inputs, then n outputs, at `off` floats into the pool
+struct MapTable {
+	int off = 0, n = 0;
+	uint64_t hash = 0; // FNV-1a over n and the points: the fingerprint a stream record carries
+	std::vector<float> pts;
+};
+static MapTable make_table(int n, const float *in, const float *out) {
+	MapTable t;
+	t.n = n;
+	t.pts.assign(in, in + n);
+	t.pts.insert(t.pts.end(), out, out + n);
+	uint64_t h = 1469598103934665603ull;
+	auto mix = [&](const void *p, size_t bytes) {
+		for (size_t i = 0; i < bytes; ++i) h = (h ^ ((const unsigned char *)p)[i]) * 1099511628211ull;
+	};
+	const int32_t n32 = n;
+	mix(&n32, sizeof(n32));
+	mix(t.pts.data(), sizeof(float) * t.pts.size());
+	t.hash = h;
+	return t;
+}
+// bit for bit (an empty table equals any other empty one)
+static bool same_points(const MapTable &a, const MapTable &b) {
+	return a.n == b.n && (a.n == 0 || (a.hash == b.hash && !memcmp(a.pts.data(), b.pts.data(), sizeof(float) * a.pts.size())));
+}
+
 struct b200s_engine {
 	int S = 0, device = 0;
 	long seed = 0;
 	bool configured = false;
 	Cfg cfg;
-	FreqMap fmap; // the custom frequency map table (mapN; its device rows are dMapIn / dMapOut)
+	// Frequency-map tables (DESIGN.md §3.9): the engine's table (b200s_set_freq_map_table; n = 0: none) and every stream's
+	// own table (b200s_set_freq_map_table_per_stream) lie de-duplicated by content in one device pool, dMaps.  `maps` holds
+	// the host copies in pool order; a stream finds its table by StreamParams::mapOff / mapN.
+	MapTable engMap;
+	std::vector<MapTable> maps;
+	float *dMaps = 0;
+	size_t mapsCap = 0, mapsUsed = 0; // floats
 	// per-stream parameters: the host table (what the setters write) and its device copy Ctx::sprm, uploaded by the next
 	// process() when dirty; the counts over the table decide which kernels a call launches
 	std::vector<StreamParams> hSprm;
@@ -99,7 +133,6 @@ struct b200s_engine {
 	float2 *dRot = 0, *dTwiddle = 0, *dPretw = 0;
 	float4 *dAnaTab = 0;
 	float2 rot0, rotStep;
-	float *dMapIn = 0, *dMapOut = 0;
 	// state
 	Sched *dSched = 0;
 	float *dHist[2] = {0, 0};
@@ -149,7 +182,6 @@ struct b200s_engine {
 	cudaEvent_t evIdx[2] = {0, 0};
 	int idxSlot = 0;
 	cudaEvent_t evXfer = 0;
-	std::vector<float> hMapIn, hMapOut; // host copy of the frequency-map table: a stream that uses it may only go to an engine with the same table
 };
 
 #define CK(call)                                                                                   \
@@ -222,9 +254,7 @@ static Ctx make_ctx(b200s_engine *e) {
 	Ctx x;
 	memset(&x, 0, sizeof(x));
 	x.cfg = e->cfg;
-	x.fmap.mapN = e->fmap.mapN;
-	x.fmap.mapIn = e->dMapIn;
-	x.fmap.mapOut = e->dMapOut;
+	x.maps = e->dMaps;
 	x.sprm = e->dSprm;
 	x.window = e->dWindow; x.winProd = e->dWinProd; x.wpReset = e->dWpReset; x.wpDiv = e->dWpDiv;
 	x.rot = e->dRot; x.twiddle = e->dTwiddle; x.pretw = e->dPretw; x.anaTab = e->dAnaTab;
@@ -798,7 +828,7 @@ static void count_paths(b200s_engine *e) {
 	e->nMapped = 0;
 	e->anyFormants = e->anyAutoPitch = false;
 	for (const StreamParams &p : e->hSprm) {
-		const bool mapped = stream_mapped(p, e->fmap.mapN), formants = stream_formants(p, mapped);
+		const bool mapped = stream_mapped(p), formants = stream_formants(p, mapped);
 		e->nMapped += (mapped || formants) ? 1 : 0;
 		e->anyFormants = e->anyFormants || formants;
 		e->anyAutoPitch = e->anyAutoPitch || (formants && !(p.formantBaseFreq > 0));
@@ -807,6 +837,85 @@ static void count_paths(b200s_engine *e) {
 static void params_changed(b200s_engine *e) {
 	count_paths(e);
 	e->sprmDirty = true;
+}
+
+// ---- the frequency-map pool ----
+// the table a stream's descriptor points at (null: none)
+static const MapTable *stream_table(const b200s_engine *e, const StreamParams &p) {
+	if (p.mapN == 0) return nullptr;
+	return &*std::lower_bound(e->maps.begin(), e->maps.end(), p.mapOff, [](const MapTable &t, int off) { return t.off < off; });
+}
+// The whole pool from the host copies, grown (to at least twice its capacity) when it has no room.  The caller has
+// synchronised the handle's stream: kernels in flight may read the pool.
+static int upload_maps(b200s_engine *e) {
+	int rc;
+	if (e->mapsUsed > e->mapsCap) {
+		const size_t cap = std::max(e->mapsUsed, 2 * e->mapsCap);
+		if ((rc = dalloc(e, &e->dMaps, cap))) return rc;
+		e->mapsCap = cap;
+	}
+	if (e->mapsUsed == 0) return 0;
+	std::vector<float> all(e->mapsUsed);
+	for (const MapTable &t : e->maps) std::copy(t.pts.begin(), t.pts.end(), all.begin() + t.off);
+	CK(cudaMemcpy(e->dMaps, all.data(), sizeof(float) * all.size(), cudaMemcpyHostToDevice));
+	return 0;
+}
+// Lays the pool out afresh from the tables in use and uploads it: the engine's table, then each stream's (the engine's
+// for kMapEngine; for kMapOwn want[s] when given, otherwise the one it has).  Tables nobody uses any more are dropped.
+// Synchronises the handle's stream.
+static int layout_maps(b200s_engine *e, const std::vector<const MapTable *> &want) {
+	CK(cudaStreamSynchronize(e->stream));
+	std::vector<MapTable> pool;
+	std::unordered_map<uint64_t, std::vector<size_t>> byHash;
+	size_t used = 0;
+	auto intern = [&](const MapTable &t) {
+		for (size_t i : byHash[t.hash])
+			if (same_points(pool[i], t)) return pool[i].off;
+		byHash[t.hash].push_back(pool.size());
+		pool.push_back(t);
+		pool.back().off = (int)used;
+		used += t.pts.size();
+		return pool.back().off;
+	};
+	if (e->engMap.n > 0) e->engMap.off = intern(e->engMap);
+	std::vector<StreamParams> prm = e->hSprm;
+	for (int s = 0; s < e->S; ++s) {
+		StreamParams &p = prm[s];
+		const MapTable *t = p.customMap == kMapEngine ? (e->engMap.n > 0 ? &e->engMap : nullptr)
+		                    : p.customMap == kMapOwn  ? (want.empty() || !want[s] ? stream_table(e, p) : want[s])
+		                                              : nullptr;
+		p.mapOff = t ? intern(*t) : 0;
+		p.mapN = t ? t->n : 0;
+		if (used > (size_t)INT_MAX) {
+			e->err = "frequency-map tables: more than 2^31-1 floats in all";
+			return B200S_EINVAL;
+		}
+	}
+	e->maps = std::move(pool);
+	e->mapsUsed = used;
+	e->hSprm = std::move(prm);
+	params_changed(e);
+	return upload_maps(e);
+}
+static cudaError_t copy_peer(void *dst, int dstDevice, const void *src, int srcDevice, size_t bytes, cudaStream_t st);
+// The table of a stream that comes from another engine, in dst's pool: found there by content, or appended and copied
+// from src's pool on dst's stream (no host synchronisation).  Growing the pool synchronises dst and uploads it whole.
+static int carry_table(b200s_engine *dst, const b200s_engine *src, const MapTable &t, int *off) {
+	b200s_engine *e = dst;
+	for (const MapTable &m : dst->maps)
+		if (same_points(m, t)) {
+			*off = m.off;
+			return 0;
+		}
+	dst->maps.push_back(t);
+	*off = dst->maps.back().off = (int)dst->mapsUsed;
+	dst->mapsUsed += t.pts.size();
+	if (dst->mapsUsed <= dst->mapsCap) {
+		CK(copy_peer(dst->dMaps + *off, dst->device, src->dMaps + t.off, src->device, sizeof(float) * t.pts.size(), dst->stream));
+		return 0;
+	}
+	CK(cudaStreamSynchronize(dst->stream));
+	return upload_maps(dst);
 }
 // Complex coefficient rows of k_prep (32 B per bin-channel and block: 6.6 GB at batch 1024 x 33 blocks stereo): only calls
 // with a stream that has a frequency map or formant processing launch k_prep, so only they pay for them (b200s_reserve()
@@ -1400,14 +1509,15 @@ struct StreamRecordHeader {
 	uint32_t version;  // kRecordVersion
 	uint32_t bytes;    // record size
 	int32_t C, B, H, split, K;
-	uint32_t flags;    // kRecPrevRandom | kRecSeekRandom | kRecUsesTable
-	int32_t mapN;      // the frequency-map table the stream uses (kRecUsesTable): its points and fingerprint
+	uint32_t flags;    // kRecPrevRandom | kRecSeekRandom | (kRecUsesTable or kRecOwnTable)
+	int32_t mapN;      // the frequency-map table the stream uses (kRecUsesTable, kRecOwnTable): its points and fingerprint
 	uint64_t mapHash;
-	StreamParams params;
+	StreamSettings params;
 };
 static_assert(sizeof(StreamRecordHeader) <= B200S_RECORD_HEADER, "record header");
 static const uint32_t kRecordVersion = 1;
-enum { kRecPrevRandom = 1, kRecSeekRandom = 2, kRecUsesTable = 4 };
+// kRecUsesTable: the stream uses the engine's table; kRecOwnTable: it has its own
+enum { kRecPrevRandom = 1, kRecSeekRandom = 2, kRecUsesTable = 4, kRecOwnTable = 8 };
 
 static StateRegions state_regions(const b200s_engine *e) {
 	const Cfg &g = e->cfg;
@@ -1435,23 +1545,9 @@ static StateRegions state_regions(const b200s_engine *e) {
 	t.recBytes = off;
 	return t;
 }
-static bool uses_table(const b200s_engine *e, const StreamParams &p) { return p.customMap && e->fmap.mapN > 0; }
-static bool same_table(const b200s_engine *a, const b200s_engine *b) {
-	const size_t n = a->hMapIn.size();
-	return a->fmap.mapN == b->fmap.mapN && b->hMapIn.size() == n && b->hMapOut.size() == n &&
-	       (n == 0 || (!memcmp(a->hMapIn.data(), b->hMapIn.data(), sizeof(float) * n) && !memcmp(a->hMapOut.data(), b->hMapOut.data(), sizeof(float) * n)));
-}
-static uint64_t table_hash(const b200s_engine *e) { // FNV-1a over the points
-	uint64_t h = 1469598103934665603ull;
-	auto mix = [&](const void *p, size_t n) {
-		for (size_t i = 0; i < n; ++i) h = (h ^ ((const unsigned char *)p)[i]) * 1099511628211ull;
-	};
-	const int32_t n = e->fmap.mapN;
-	mix(&n, sizeof(n));
-	mix(e->hMapIn.data(), sizeof(float) * e->hMapIn.size());
-	mix(e->hMapOut.data(), sizeof(float) * e->hMapOut.size());
-	return h;
-}
+// the stream uses the engine's table (a stream with its own table is kMapOwn)
+static bool uses_table(const b200s_engine *e, const StreamParams &p) { return p.customMap == kMapEngine && e->engMap.n > 0; }
+static bool same_table(const b200s_engine *a, const b200s_engine *b) { return same_points(a->engMap, b->engMap); }
 static bool same_config(const Cfg &a, const Cfg &b) { return a.C == b.C && a.B == b.B && a.H == b.H && a.split == b.split; }
 static std::string cfg_text(const Cfg &g) {
 	return std::to_string(g.C) + " channels, block " + std::to_string(g.B) + ", interval " + std::to_string(g.H) + (g.split ? ", split" : "");
@@ -1547,8 +1643,9 @@ struct DeviceGuard {
 		if (prev >= 0) cudaSetDevice(prev);
 	}
 };
-// packed records from one device to another, without peer access enabled (the emulator has one device: never called)
-static cudaError_t copy_records_peer(char *dst, int dstDevice, const char *src, int srcDevice, size_t bytes, cudaStream_t st) {
+// packed records or a frequency-map table from one engine's device to another's (the same or another device), without peer
+// access enabled (the emulator has one device)
+static cudaError_t copy_peer(void *dst, int dstDevice, const void *src, int srcDevice, size_t bytes, cudaStream_t st) {
 #ifdef B200S_EMU
 	(void)dstDevice;
 	(void)srcDevice;
@@ -1595,6 +1692,10 @@ static int copy_impl(b200s_engine *dst, const int *dstS, b200s_engine *src, cons
 		if ((rc = launch_pack(src, n))) return rc;
 		if (!same) CK(cudaEventRecord(src->evXfer, src->stream));
 	}
+	// parameters through the host table (read before any is written: swaps and forks), uploaded by the next call.  Within
+	// one engine a stream keeps its table descriptor; across engines it points into the destination's pool.
+	std::vector<StreamParams> p((size_t)n);
+	for (int i = 0; i < n; ++i) p[i] = src->hSprm[srcS[i]];
 	if (same) {
 		if ((rc = launch_unpack(dst, n, dst->dXfer))) return rc;
 	} else {
@@ -1604,21 +1705,25 @@ static int copy_impl(b200s_engine *dst, const int *dstS, b200s_engine *src, cons
 		if ((rc = upload_lists(dst, nullptr, dstS, n))) return rc;
 		CK(cudaStreamWaitEvent(dst->stream, src->evXfer, 0));
 		const size_t bytes = (size_t)n * state_regions(src).recBytes;
-		if (peer) CK(copy_records_peer(dst->dXfer, dst->device, src->dXfer, src->device, bytes, dst->stream));
+		if (peer) CK(copy_peer(dst->dXfer, dst->device, src->dXfer, src->device, bytes, dst->stream));
 		if ((rc = launch_unpack(dst, n, peer ? dst->dXfer : src->dXfer))) return rc;
-		// the source's records are free again once the destination has read them
+		for (int i = 0; i < n; ++i) {
+			if (p[i].customMap == kMapOwn) {
+				if ((rc = carry_table(dst, src, *stream_table(src, p[i]), &p[i].mapOff))) return rc;
+			} else if (uses_table(src, p[i])) {
+				p[i].mapOff = dst->engMap.off; // (check_copy: the same table)
+			} else {
+				p[i].customMap = kMapNone;
+				p[i].mapOff = p[i].mapN = 0;
+			}
+		}
+		// the source's records and tables are free again once the destination has read them
 		CK(cudaEventRecord(dst->evXfer, dst->stream));
 		e = src;
 		CK(cudaSetDevice(src->device));
 		CK(cudaStreamWaitEvent(src->stream, dst->evXfer, 0));
 	}
 	dst->chainedGroups = 0;
-	// parameters through the host table (read before any is written: swaps and forks), uploaded by the next call
-	std::vector<StreamParams> p((size_t)n);
-	for (int i = 0; i < n; ++i) {
-		p[i] = src->hSprm[srcS[i]];
-		if (!same && !uses_table(src, p[i])) p[i].customMap = 0;
-	}
 	for (int i = 0; i < n; ++i) dst->hSprm[dstS[i]] = p[i];
 	params_changed(dst);
 	dst->prevCallMayRandom = dst->prevCallMayRandom || src->prevCallMayRandom;
@@ -1649,7 +1754,6 @@ int b200s_create(int batch, long seed, int device, b200s_engine **out) {
 	e->seed = seed;
 	e->device = device;
 	memset(&e->cfg, 0, sizeof(e->cfg));
-	memset(&e->fmap, 0, sizeof(e->fmap));
 	{
 		StreamParams p;
 		memset(&p, 0, sizeof(p));
@@ -1712,8 +1816,7 @@ void b200s_destroy(b200s_engine *e) {
 	cudaSetDevice(e->device);
 	cudaStreamSynchronize(e->stream);
 	free_all(e);
-	dfree(e->dMapIn);
-	dfree(e->dMapOut);
+	dfree(e->dMaps);
 	dfree(e->dRng);
 	dfree(e->dDiag);
 	dfree(e->dSeekStf);
@@ -1842,7 +1945,8 @@ static void set_transpose(StreamParams &p, float multiplier, float tonality) { /
 	p.freqMultiplier = multiplier;
 	if (tonality > 0) p.freqTonalityLimit = tonality / std::sqrt(multiplier);
 	else p.freqTonalityLimit = 1;
-	p.customMap = 0; // (setTransposeFactor clears customFreqMap)
+	p.customMap = kMapNone; // (setTransposeFactor clears customFreqMap)
+	p.mapOff = p.mapN = 0;
 }
 static float semitones_factor(float semitones) { return std::pow(2, semitones / 12); } // :116-118, :129-131
 static void set_formant(StreamParams &p, float multiplier, int comp) { // :124-128
@@ -1907,23 +2011,41 @@ int b200s_set_formant_base_per_stream(b200s_engine *e, const float *base) {
 }
 int b200s_set_freq_map_table(b200s_engine *e, const float *fin, const float *fout, int n) {
 	if (!e || n < 0 || (n > 0 && (!fin || !fout))) return B200S_EINVAL;
-	CK(cudaStreamSynchronize(e->stream));
-	dfree(e->dMapIn);
-	dfree(e->dMapOut);
-	e->fmap.mapN = 0;
-	e->hMapIn.assign(fin, fin + n);
-	e->hMapOut.assign(fout, fout + n);
-	for (StreamParams &p : e->hSprm) p.customMap = 1; // one table per engine, used by every stream until a transpose setter
-	params_changed(e);
+	e->engMap = make_table(n, fin, fout);
+	for (StreamParams &p : e->hSprm) p.customMap = kMapEngine; // every stream, until a transpose setter or its own table
+	return layout_maps(e, {});
+}
+int b200s_set_freq_map_table_per_stream(b200s_engine *e, const int *streams, int n, const int *n_points, const float *fin, const float *fout) {
+	if (!e) return B200S_EINVAL;
+	std::string why;
+	if (n < 0) why = "negative stream count";
+	else if (n > 0 && (!streams || !n_points)) why = std::string(streams ? "n_points" : "streams") + " must not be NULL";
+	long long total = 0;
+	std::vector<char> seen((size_t)e->S, 0);
+	for (int i = 0; i < n && why.empty(); ++i) {
+		const int s = streams[i];
+		const std::string at = "streams[" + std::to_string(i) + "]";
+		if (s < 0 || s >= e->S) why = at + " = " + std::to_string(s) + " is outside [0, " + std::to_string(e->S) + ")";
+		else if (seen[s]++) why = at + ": stream " + std::to_string(s) + " is listed twice";
+		else if (n_points[i] < 0) why = "n_points[" + std::to_string(i) + "] = " + std::to_string(n_points[i]) + " is negative";
+		else total += n_points[i];
+	}
+	if (why.empty() && total > 0 && (!fin || !fout)) why = "freq_in and freq_out must not be NULL";
+	if (!why.empty()) {
+		e->err = "b200s_set_freq_map_table_per_stream: " + why;
+		return B200S_EINVAL;
+	}
 	if (n == 0) return 0;
-	int rc;
-	if ((rc = dalloc(e, &e->dMapIn, n))) return rc;
-	if ((rc = dalloc(e, &e->dMapOut, n))) return rc;
-	CK(cudaMemcpy(e->dMapIn, fin, sizeof(float) * n, cudaMemcpyHostToDevice));
-	CK(cudaMemcpy(e->dMapOut, fout, sizeof(float) * n, cudaMemcpyHostToDevice));
-	e->fmap.mapN = n;
-	params_changed(e);
-	return 0;
+	std::vector<MapTable> tabs((size_t)n);
+	std::vector<const MapTable *> want((size_t)e->S, nullptr);
+	for (long long i = 0, at = 0; i < n; at += n_points[i++]) {
+		StreamParams &p = e->hSprm[streams[i]];
+		p.customMap = n_points[i] > 0 ? kMapOwn : kMapNone;
+		if (n_points[i] == 0) continue;
+		tabs[i] = make_table(n_points[i], fin + at, fout + at);
+		want[streams[i]] = &tabs[i];
+	}
+	return layout_maps(e, want);
 }
 
 int b200s_seek_device(b200s_engine *e, const float *dIn, int n, double rate) {
@@ -2240,7 +2362,6 @@ int b200s_export_streams(b200s_engine *e, const int *streams, int n, void *host_
 	const size_t R = state_regions(e).recBytes;
 	CK(cudaMemcpyAsync(host_dst, e->dXfer, (size_t)n * R, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
-	const uint64_t hash = table_hash(e);
 	for (int i = 0; i < n; ++i) {
 		StreamRecordHeader h;
 		memset(&h, 0, sizeof(h));
@@ -2248,14 +2369,16 @@ int b200s_export_streams(b200s_engine *e, const int *streams, int n, void *host_
 		h.version = kRecordVersion;
 		h.bytes = (uint32_t)R;
 		h.C = e->cfg.C; h.B = e->cfg.B; h.H = e->cfg.H; h.split = e->cfg.split; h.K = e->cfg.K;
-		h.params = e->hSprm[streams[i]];
+		const StreamParams &p = e->hSprm[streams[i]];
+		h.params = p;
 		h.flags = (e->prevCallMayRandom ? kRecPrevRandom : 0) | (e->seekMayRandom ? kRecSeekRandom : 0);
-		if (uses_table(e, h.params)) {
-			h.flags |= kRecUsesTable;
-			h.mapN = e->fmap.mapN;
-			h.mapHash = hash;
+		const MapTable *t = uses_table(e, p) ? &e->engMap : p.customMap == kMapOwn ? stream_table(e, p) : nullptr;
+		if (t) {
+			h.flags |= uses_table(e, p) ? kRecUsesTable : kRecOwnTable;
+			h.mapN = t->n;
+			h.mapHash = t->hash;
 		} else {
-			h.params.customMap = 0;
+			h.params.customMap = kMapNone;
 		}
 		char *rec = (char *)host_dst + (size_t)i * R;
 		memset(rec, 0, B200S_RECORD_HEADER);
@@ -2272,19 +2395,32 @@ int b200s_import_streams(b200s_engine *e, const int *streams, int n, const void 
 	}
 	if (!check_streams(e->err, fn, "streams", streams, n, e->S, true)) return B200S_EINVAL;
 	const size_t R = state_regions(e).recBytes;
-	const uint64_t hash = table_hash(e);
 	std::vector<StreamRecordHeader> hs((size_t)n);
+	std::vector<StreamParams> prm((size_t)n); // the streams' parameters after the import, table descriptors included
 	for (int i = 0; i < n; ++i) {
 		StreamRecordHeader &h = hs[i];
 		memcpy(&h, (const char *)host_src + (size_t)i * R, sizeof(h));
+		// a stream with its own table goes into a slot that holds the same table already (its own or the engine's)
+		const MapTable *slot = stream_table(e, e->hSprm[streams[i]]);
 		std::string why;
 		if (memcmp(h.magic, "B200SREC", 8)) why = "not a stream record";
 		else if (h.version != kRecordVersion) why = "record format " + std::to_string(h.version) + ", this library reads " + std::to_string(kRecordVersion);
 		else if (h.C != e->cfg.C || h.B != e->cfg.B || h.H != e->cfg.H || h.split != e->cfg.split || h.K != e->cfg.K || h.bytes != R)
 			why = "recorded with another configuration (" + std::to_string(h.C) + " channels, block " + std::to_string(h.B) + ", interval " +
 			      std::to_string(h.H) + (h.split ? ", split" : "") + "; this engine: " + cfg_text(e->cfg) + ")";
-		else if ((h.flags & kRecUsesTable) && (h.mapN != e->fmap.mapN || h.mapHash != hash))
+		else if ((h.flags & ~(uint32_t)(kRecPrevRandom | kRecSeekRandom | kRecUsesTable | kRecOwnTable)) ||
+		         ((h.flags & kRecUsesTable) && (h.flags & kRecOwnTable)))
+			why = "unknown flags " + std::to_string(h.flags);
+		else if ((h.flags & kRecUsesTable) && (h.mapN != e->engMap.n || h.mapHash != e->engMap.hash))
 			why = "the stream uses a frequency-map table that differs from this engine's";
+		else if ((h.flags & kRecOwnTable) && !(slot && h.mapN == slot->n && h.mapHash == slot->hash))
+			why = "the stream has its own frequency-map table, and slot " + std::to_string(streams[i]) + " does not hold the same table";
+		StreamParams &p = prm[i];
+		static_cast<StreamSettings &>(p) = h.params;
+		const MapTable *t = (h.flags & kRecUsesTable) ? &e->engMap : (h.flags & kRecOwnTable) ? slot : nullptr;
+		p.customMap = (h.flags & kRecUsesTable) ? kMapEngine : (h.flags & kRecOwnTable) ? kMapOwn : kMapNone;
+		p.mapOff = t ? t->off : 0;
+		p.mapN = t ? t->n : 0;
 		if (!why.empty()) {
 			e->err = std::string(fn) + ": record " + std::to_string(i) + ": " + why;
 			return B200S_EINVAL;
@@ -2300,7 +2436,7 @@ int b200s_import_streams(b200s_engine *e, const int *streams, int n, const void 
 	e->chainedGroups = 0;
 	if ((rc = launch_unpack(e, n, e->dXfer))) return rc;
 	for (int i = 0; i < n; ++i) {
-		e->hSprm[streams[i]] = hs[i].params;
+		e->hSprm[streams[i]] = prm[i];
 		e->prevCallMayRandom = e->prevCallMayRandom || (hs[i].flags & kRecPrevRandom);
 		e->seekMayRandom = e->seekMayRandom || (hs[i].flags & kRecSeekRandom);
 	}
@@ -2322,9 +2458,12 @@ int b200s_clone(b200s_engine *src, b200s_engine **out) {
 	}
 	e->chainV = src->chainV; e->fftV1 = src->fftV1; e->nHostParts = src->nHostParts; e->exactMath = src->exactMath;
 	e->stepMajor = src->stepMajor; e->dual = src->dual; e->nSub = src->nSub;
-	const int mapN = src->fmap.mapN;
-	if (mapN > 0 && (rc = b200s_set_freq_map_table(e, src->hMapIn.data(), src->hMapOut.data(), mapN))) goto fail;
-	e->hSprm = src->hSprm; // (setting the table turned it on for every stream)
+	// the frequency-map pool as the source lays it out, so that every stream's table descriptor holds as it is
+	e->engMap = src->engMap;
+	e->maps = src->maps;
+	e->mapsUsed = src->mapsUsed;
+	if ((rc = upload_maps(e))) goto fail;
+	e->hSprm = src->hSprm;
 	params_changed(e);
 	if (src->configured) {
 		std::vector<int> all((size_t)src->S);
