@@ -200,6 +200,29 @@ int b200s_run_per_stream_async(b200s_engine *e, const int *ops, const float *in,
                                float *out, int out_stride, const int *output_samples, const double *playback_rates);
 int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *d_in, int in_stride, const int *input_samples,
                                 float *d_out, int out_stride, const int *output_samples, const double *playback_rates);
+/* b200s_run_per_stream over a list of streams: a server whose batch has 1024 slots and 100 active sessions moves and
+ * processes 100 rows per call, not 1024.  Entry i belongs to stream streams[i], which runs ops[i] with input_samples[i],
+ * output_samples[i] and playback_rates[i]; the buffers are packed over the list, [n][channels][stride], row i for stream
+ * streams[i], and every array holds n entries.  The slots may be listed in any order.
+ *   - A listed stream is bit-identical to what b200s_run_per_stream does with the same op at its slot, outputs and state;
+ *     every output sample its op does not produce is written as zero, up to out_stride.
+ *   - A stream that is not listed is neither read nor written: its state stays unchanged, byte for byte (SKIP without an
+ *     output row).  n == 0 enqueues nothing.
+ *   - B200S_EINVAL before anything is enqueued, b200s_last_error() naming the entry: n < 0 or n > batch, NULL streams, ops
+ *     or count arrays with n > 0, a slot outside [0, batch) or listed twice, and every rule of b200s_run_per_stream.
+ *   - b200s_reserve(in_stride, out_stride) sizes these calls as it sizes b200s_run_per_stream: no allocation afterwards.
+ *   - Host buffers: a call of PROCESS / SKIP ops pipelines like b200s_run_per_stream_async when the previous call ran over
+ *     the same list (the same slots in the same order) with the same strides; any other call joins.
+ *   b200s_run_streams: host buffers, synchronous; _async: host buffers, returns once enqueued; _device: device buffers,
+ *   asynchronous on the handle's stream.  The arrays other than the buffers are host arrays, copied during the call. */
+int b200s_run_streams(b200s_engine *e, int n, const int *streams, const int *ops, const float *in, int in_stride,
+                      const int *input_samples, float *out, int out_stride, const int *output_samples, const double *playback_rates);
+int b200s_run_streams_async(b200s_engine *e, int n, const int *streams, const int *ops, const float *in, int in_stride,
+                            const int *input_samples, float *out, int out_stride, const int *output_samples,
+                            const double *playback_rates);
+int b200s_run_streams_device(b200s_engine *e, int n, const int *streams, const int *ops, const float *d_in, int in_stride,
+                             const int *input_samples, float *d_out, int out_stride, const int *output_samples,
+                             const double *playback_rates);
 
 /* ---- moving, duplicating and saving single streams ----
  * A server that rebalances streams over engines or GPUs, forks a session to preview two settings from the same point,

@@ -34,6 +34,7 @@ ABI_SYMBOLS = [
     "b200s_seek_device", "b200s_process_device", "b200s_flush_device",
     "b200s_process_per_stream", "b200s_process_per_stream_async", "b200s_process_per_stream_device",
     "b200s_run_per_stream", "b200s_run_per_stream_async", "b200s_run_per_stream_device",
+    "b200s_run_streams", "b200s_run_streams_async", "b200s_run_streams_device",
     "b200s_timer_start", "b200s_timer_stop", "b200s_kernel_launches", "b200s_device_allocations", "b200s_unserved_random_blocks", "b200s_profile_begin", "b200s_profile_end",
     "b200s_selftest_divsqrt",
     "b200s_state_size", "b200s_get_state", "b200s_set_state",
@@ -107,6 +108,9 @@ def _bind(lib):
         "b200s_run_per_stream": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
         "b200s_run_per_stream_async": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
         "b200s_run_per_stream_device": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
+        "b200s_run_streams": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
+        "b200s_run_streams_async": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
+        "b200s_run_streams_device": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
         "b200s_timer_start": (ci, [vp]), "b200s_timer_stop": (ci, [vp, fp]), "b200s_kernel_launches": (cll, [vp]), "b200s_device_allocations": (cll, [vp]), "b200s_unserved_random_blocks": (cll, [vp]),
         "b200s_profile_begin": (ci, [vp]), "b200s_profile_end": (ci, [vp, fp, ip, ci]),
         "b200s_selftest_divsqrt": (ci, [vp, cll, cll, ctypes.POINTER(cll), ctypes.POINTER(cll)]),
@@ -317,11 +321,11 @@ class BatchStretch:
                                                                ain.ctypes.data_as(fp), aout.ctypes.data_as(fp)))
 
     # ---- the hot path ----
-    def _shape(self, n):
+    def _shape(self, n, rows=None):
         c = self.channels()
         if c <= 0:
             raise StretchError("engine not configured: call presetDefault / presetCheaper / configure first")
-        return (self.batch, c, n)
+        return (self.batch if rows is None else rows, c, n)
 
     def _adopt_torch_stream(self):
         """Device-pointer calls are enqueued on torch's CURRENT stream (b200s_set_stream), so they are ordered after the
@@ -366,26 +370,28 @@ class BatchStretch:
         x = _host(x, self._shape(n))
         self._ck(self._lib.b200s_output_seek(self._h, x.ctypes.data, n))
 
-    def _lengths(self, v, name):
-        """One sample count per stream as a contiguous int32 array (a scalar is repeated)."""
+    def _lengths(self, v, name, rows=None):
+        """One sample count per stream (or per entry of a list of `rows` streams) as a contiguous int32 array (a scalar is
+        repeated)."""
+        rows = self.batch if rows is None else rows
         a = np.asarray(v)
         if a.ndim == 0:
-            a = np.full(self.batch, int(a))
-        if a.shape != (self.batch,):
-            raise ValueError("%s: expected a scalar or %d values (one per stream), got shape %s" % (name, self.batch, np.shape(v)))
+            a = np.full(rows, int(a))
+        if a.shape != (rows,):
+            raise ValueError("%s: expected a scalar or %d values (one per stream), got shape %s" % (name, rows, np.shape(v)))
         if not np.issubdtype(a.dtype, np.integer):
             raise ValueError("%s: expected integer sample counts, got %s" % (name, a.dtype))
         return np.ascontiguousarray(a, np.int32)
 
-    def process(self, inputs, outputSamples, out=None, inputSamples=None):
+    def process(self, inputs, outputSamples, out=None, inputSamples=None, streams=None):
         """inputs: [batch][channels][inputSamples] (numpy -> host API; torch CUDA tensor -> device API).
 
         outputSamples: an int, or one per stream; inputSamples: None (every stream reads all of `inputs`' last dimension)
         or one per stream.  With any per-stream array, stream s reads the first inputSamples[s] samples of its rows and
         writes the first outputSamples[s] of an output of max(outputSamples) samples per row, zeros after them
-        (b200s_process_per_stream)."""
-        if np.ndim(outputSamples) > 0 or inputSamples is not None:
-            return self._process_per_stream(inputs, outputSamples, out, inputSamples)
+        (b200s_process_per_stream).  streams: only these streams process, as in run()."""
+        if np.ndim(outputSamples) > 0 or inputSamples is not None or streams is not None:
+            return self.run(self.OP_PROCESS, inputs, outputSamples, inputSamples=inputSamples, out=out, streams=streams)
         if _is_torch_cuda(inputs):
             import torch
 
@@ -404,66 +410,71 @@ class BatchStretch:
         self._ck(self._lib.b200s_process(self._h, x.ctypes.data, n_in, out.ctypes.data, outputSamples))
         return out
 
-    def _process_per_stream(self, inputs, outputSamples, out, inputSamples):
-        return self.run(self.OP_PROCESS, inputs, outputSamples, inputSamples=inputSamples, out=out)
-
-    def run(self, ops, inputs, outputSamples, inputSamples=None, playbackRates=None, out=None):
+    def run(self, ops, inputs, outputSamples, inputSamples=None, playbackRates=None, out=None, streams=None):
         """Every stream runs its own operation (b200s_run_per_stream): ops, outputSamples, inputSamples and playbackRates are
         scalars (repeated for every stream) or one value per stream.  OP_PROCESS: process(inputs[s][:, :inputSamples[s]],
         outputSamples[s]); OP_SEEK: seek(inputs[s][:, :inputSamples[s]], playbackRates[s]); OP_OUTPUT_SEEK:
         outputSeek(inputs[s][:, :inputSamples[s]]); OP_FLUSH: flush(outputSamples[s], playbackRates[s]); OP_RESET: reset();
         OP_SKIP: nothing.  inputs: [batch][channels][stride] (numpy -> host API; torch CUDA tensor -> device API; None
         when no stream reads input); inputSamples defaults to the whole stride for the ops that read input and 0 for the
-        others.  Returns [batch][channels][max(outputSamples)] (or `out`), zeros after each stream's own output."""
+        others.  Returns [batch][channels][max(outputSamples)] (or `out`), zeros after each stream's own output.
+
+        streams: a list of n slots (b200s_run_streams).  Only they run; every array then has one value per list entry and
+        the buffers are [n][channels][stride], row i for stream streams[i].  The other streams are not touched."""
         torch_in = _is_torch_cuda(inputs)
-        op = self._lengths(ops, "ops")
+        lst = None if streams is None else self._stream_list(streams, "streams")
+        rows = self.batch if lst is None else int(lst.size)
+        op = self._lengths(ops, "ops", rows)
         if np.any((op < 0) | (op > 5)):
             raise ValueError("ops: every op must be one of OP_SKIP .. OP_RESET")
-        n_out = self._lengths(outputSamples, "outputSamples")
+        n_out = self._lengths(outputSamples, "outputSamples", rows)
         in_stride = 0 if inputs is None else int(inputs.shape[-1]) if torch_in else int(np.shape(inputs)[-1])
         if inputSamples is None:
             reads = (op == self.OP_PROCESS) | (op == self.OP_SEEK) | (op == self.OP_OUTPUT_SEEK)
             inputSamples = np.where(reads, in_stride, 0)
-        n_in = self._lengths(inputSamples, "inputSamples")
+        n_in = self._lengths(inputSamples, "inputSamples", rows)
         rates = None
         if playbackRates is not None:
-            rates = np.ascontiguousarray(np.broadcast_to(np.asarray(playbackRates, np.float64), (self.batch,)) if np.ndim(playbackRates) == 0
+            rates = np.ascontiguousarray(np.broadcast_to(np.asarray(playbackRates, np.float64), (rows,)) if np.ndim(playbackRates) == 0
                                          else np.asarray(playbackRates, np.float64))
-            if rates.shape != (self.batch,):
-                raise ValueError("playbackRates: expected a scalar or %d values, got shape %s" % (self.batch, np.shape(playbackRates)))
-        out_stride = int(n_out.max()) if self.batch else 0
+            if rates.shape != (rows,):
+                raise ValueError("playbackRates: expected a scalar or %d values, got shape %s" % (rows, np.shape(playbackRates)))
+        out_stride = int(n_out.max()) if rows else 0
         if out is not None:
             out_stride = int(out.shape[-1])
-            if tuple(out.shape) != self._shape(out_stride):
-                raise ValueError("out: expected shape %s, got %s" % (self._shape(out_stride), tuple(out.shape)))
+            if tuple(out.shape) != self._shape(out_stride, rows):
+                raise ValueError("out: expected shape %s, got %s" % (self._shape(out_stride, rows), tuple(out.shape)))
         for name, a, stride in (("inputSamples", n_in, in_stride), ("outputSamples", n_out, out_stride)):
             bad = np.flatnonzero((a < 0) | (a > stride))
             if bad.size:
                 raise ValueError("%s[%d] = %d is outside [0, %d]" % (name, bad[0], a[bad[0]], stride))
         ip, dp = ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_double)
         rp = None if rates is None else rates.ctypes.data_as(dp)
+
+        def call(fn_all, fn_list, in_ptr, out_ptr):
+            args = (op.ctypes.data_as(ip), in_ptr, in_stride, n_in.ctypes.data_as(ip), out_ptr, out_stride, n_out.ctypes.data_as(ip), rp)
+            self._ck(fn_all(self._h, *args) if lst is None else fn_list(self._h, rows, lst.ctypes.data_as(ip), *args))
+
         if torch_in:
             import torch
 
             self._adopt_torch_stream()
             assert inputs.is_contiguous() and inputs.dtype == torch.float32
-            if tuple(inputs.shape) != self._shape(in_stride):
-                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), tuple(inputs.shape)))
+            if tuple(inputs.shape) != self._shape(in_stride, rows):
+                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride, rows), tuple(inputs.shape)))
             if out is None:
-                out = torch.empty(self._shape(out_stride), dtype=torch.float32, device=inputs.device)
-            self._ck(self._lib.b200s_run_per_stream_device(self._h, op.ctypes.data_as(ip), inputs.data_ptr(), in_stride, n_in.ctypes.data_as(ip),
-                                                           out.data_ptr(), out_stride, n_out.ctypes.data_as(ip), rp))
+                out = torch.empty(self._shape(out_stride, rows), dtype=torch.float32, device=inputs.device)
+            call(self._lib.b200s_run_per_stream_device, self._lib.b200s_run_streams_device, inputs.data_ptr(), out.data_ptr())
             return out
         x = None
         if inputs is not None:
             x = np.asarray(inputs, np.float32)
-            if x.shape != self._shape(in_stride):
-                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride), x.shape))
-            x = _host(x, self._shape(in_stride))
+            if x.shape != self._shape(in_stride, rows):
+                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride, rows), x.shape))
+            x = _host(x, self._shape(in_stride, rows))
         if out is None:
-            out = np.empty(self._shape(out_stride), np.float32)
-        self._ck(self._lib.b200s_run_per_stream(self._h, op.ctypes.data_as(ip), None if x is None else x.ctypes.data, in_stride,
-                                                n_in.ctypes.data_as(ip), out.ctypes.data, out_stride, n_out.ctypes.data_as(ip), rp))
+            out = np.empty(self._shape(out_stride, rows), np.float32)
+        call(self._lib.b200s_run_per_stream, self._lib.b200s_run_streams, None if x is None else x.ctypes.data, out.ctypes.data)
         return out
 
     def process_per_stream_host_ptr(self, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, wait=False):
@@ -485,6 +496,19 @@ class BatchStretch:
         rp = None if r is None else r.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
         fn = self._lib.b200s_run_per_stream if wait else self._lib.b200s_run_per_stream_async
         self._ck(fn(self._h, o.ctypes.data_as(ip), in_ptr, int(in_stride), a.ctypes.data_as(ip), out_ptr, int(out_stride), b.ctypes.data_as(ip), rp))
+
+    def run_streams_host_ptr(self, streams, ops, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, playback_rates=None, wait=False):
+        """run_per_stream_host_ptr over a list of streams (b200s_run_streams / _async): pinned buffers [n][channels][stride],
+        row i and the i-th value of ops, counts and rates for stream streams[i]."""
+        ip = ctypes.POINTER(ctypes.c_int)
+        lst = self._stream_list(streams, "streams")
+        n = int(lst.size)
+        o, a, b = self._lengths(ops, "ops", n), self._lengths(n_in, "n_in", n), self._lengths(n_out, "n_out", n)
+        r = None if playback_rates is None else np.ascontiguousarray(np.broadcast_to(np.asarray(playback_rates, np.float64), (n,)))
+        rp = None if r is None else r.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+        fn = self._lib.b200s_run_streams if wait else self._lib.b200s_run_streams_async
+        self._ck(fn(self._h, n, lst.ctypes.data_as(ip), o.ctypes.data_as(ip), in_ptr, int(in_stride), a.ctypes.data_as(ip), out_ptr,
+                    int(out_stride), b.ctypes.data_as(ip), rp))
 
     def process_host_ptr(self, in_ptr, n_in, out_ptr, n_out):
         """Raw host pointers (e.g. pinned torch tensors): the end-to-end call bench.py times."""

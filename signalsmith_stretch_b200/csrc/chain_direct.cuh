@@ -37,8 +37,9 @@ __global__ void __launch_bounds__(32) k_chain_direct(Ctx x) {
 	const int K = g.K;
 	B200S_DYN_SHARED
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const int s = x.sBase + blockIdx.x * (blockDim.x >> 5) + warp;
-	if (s >= x.sBase + x.sCount) return;
+	const int pos = x.sBase + blockIdx.x * (blockDim.x >> 5) + warp;
+	if (pos >= x.sBase + x.sCount) return;
+	const int s = stream_at(x, pos);
 	const Call cl = x.call[s];
 	if (cl.nFrames == 0) return;
 	if (cl.mapped || (cl.hasRandom && x.randomPathOn)) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream

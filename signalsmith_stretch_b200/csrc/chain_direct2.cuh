@@ -64,18 +64,19 @@ __device__ __forceinline__ void spin_pause() { __nanosleep(64); }
 __device__ __forceinline__ float2 sel2b(bool p, float2 a) { return make_float2(p ? a.x : 0.f, p ? a.y : 0.f); }
 
 // k_chain_direct6<.., DUAL> (chain_direct6.cuh) packs two mono streams into one warp.  It needs both streams of the pair
-// starting at stream s (s - sBase even) to be there, free of random blocks, and to walk the same schedule in this call --
+// at positions i and i + 1 (i - sBase even; streams s = stream_at(x, i) and t = stream_at(x, i + 1), which a listed call
+// may take from anywhere in the batch) to be there, free of random blocks, and to walk the same schedule in this call --
 // same blocks, flags, time factors and spectrum slots (streams of a batch do, unless one of them was silent or sought
 // differently).  Pairs that fail run one stream at a time (the stream in both halves).
-__device__ __forceinline__ bool dual_pair_ok(const Ctx &x, int s, int lane) {
-	if (s + 1 >= x.sBase + x.sCount) return false;
-	const Call a = x.call[s], b = x.call[s + 1];
+__device__ __forceinline__ bool dual_pair_ok(const Ctx &x, int i, int s, int t, int lane) {
+	if (i + 1 >= x.sBase + x.sCount) return false;
+	const Call a = x.call[s], b = x.call[t];
 	if (a.nFrames == 0 || a.nFrames != b.nFrames || a.bypass || b.bypass) return false;
 	if ((a.hasRandom || b.hasRandom) && x.randomPathOn) return false;
 	if (a.mapped || b.mapped) return false; // a partner on the mapped path: the plain stream runs alone
 	bool bad = false;
 	for (int f = lane; f < a.nFrames; f += 32) {
-		const Frame fa = x.frames[(size_t)s * x.maxFrames + f], fb = x.frames[(size_t)(s + 1) * x.maxFrames + f];
+		const Frame fa = x.frames[(size_t)s * x.maxFrames + f], fb = x.frames[(size_t)t * x.maxFrames + f];
 		bad = bad || fa.flags != fb.flags || fa.timeFactor != fb.timeFactor || fa.inSlot != fb.inSlot || fa.prevSlot != fb.prevSlot;
 	}
 	return !__any_sync(0xffffffffu, bad);
@@ -92,7 +93,7 @@ __global__ void __launch_bounds__(32 * CH2_MAXW) k_chain_direct2(Ctx x) {
 	constexpr int D = LT + 1;    // wavefront skew between consecutive blocks (bins)
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nWarps = blockDim.x >> 5;
 	const int j = lane / CT, c = lane % CT; // block within the warp, channel
-	const int s = x.sBase + blockIdx.x;
+	const int s = stream_at(x, x.sBase + blockIdx.x);
 	const Call cl = x.call[s];
 	if (cl.nFrames == 0 || cl.mapped) return; // (streams with a frequency map or formants: the mapped path)
 	if (cl.hasRandom && x.randomPathOn) return; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream

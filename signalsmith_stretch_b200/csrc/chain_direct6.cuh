@@ -79,12 +79,15 @@ __global__ void __launch_bounds__(32) k_chain_direct6(Ctx x) {
 	const int K = g.K;
 	B200S_DYN_SHARED
 	const int lane = threadIdx.x & 31;
-	// DUAL: CTA p owns streams s0 = sBase + 2p and s0 + 1.  When they share their schedule (dual_pair_ok) they run packed,
-	// stream s0 in the low halves and s0 + 1 in the high halves; otherwise (and for the odd stream of an odd batch) each
-	// runs alone with itself in both halves, one after the other -- every mono stream goes through the same arithmetic.
-	const int s0 = x.sBase + (DUAL ? 2 : 1) * blockIdx.x;
-	const bool pairOk = DUAL && dual_pair_ok(x, s0, lane);
-	const int nPass = (DUAL && !pairOk && s0 + 1 < x.sBase + x.sCount) ? 2 : 1;
+	// DUAL: CTA p owns the streams s0, s1 at positions i0 = sBase + 2p and i0 + 1 (stream_at: a listed call pairs its list
+	// entries, wherever their streams are).  When they share their schedule (dual_pair_ok) they run packed, stream s0 in the
+	// low halves and s1 in the high halves; otherwise (and for the odd stream of an odd batch) each runs alone with itself in
+	// both halves, one after the other -- every mono stream goes through the same arithmetic.
+	const int i0 = x.sBase + (DUAL ? 2 : 1) * blockIdx.x;
+	const bool hasPartner = DUAL && i0 + 1 < x.sBase + x.sCount;
+	const int s0 = stream_at(x, i0), s1 = hasPartner ? stream_at(x, i0 + 1) : s0;
+	const bool pairOk = DUAL && dual_pair_ok(x, i0, s0, s1, lane);
+	const int nPass = (hasPartner && !pairOk) ? 2 : 1;
 	constexpr int G = LT + 2; // lane skew in bins
 	static_assert(G + 1 <= CH6_ER && 2 * CHAIN_CH <= CH6_ER, "energy ring too short");
 	Chain6Tiles &U = *(Chain6Tiles *)dyn_smem;
@@ -96,11 +99,11 @@ __global__ void __launch_bounds__(32) k_chain_direct6(Ctx x) {
 	const c2 zc = c2{z2, z2};
 
 	for (int pass = 0; pass < nPass; ++pass) {
-	const int s = s0 + pass;
+	const int s = pass ? s1 : s0;
 	const Call cl = x.call[s];
 	if (cl.nFrames == 0 || cl.mapped) continue; // (streams with a frequency map or formants: the mapped path)
 	if (cl.hasRandom && x.randomPathOn) continue; // a block beyond 2x stretch draws random time factors: k_prep + k_chain take the stream
-	const int sH[2] = {s, pairOk ? s + 1 : s};
+	const int sH[2] = {s, pairOk ? s1 : s};
 	for (int base = 0; base < cl.nFrames; base += 32) {
 		__syncwarp();
 		const int f = base + lane;

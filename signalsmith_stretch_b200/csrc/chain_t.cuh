@@ -30,7 +30,7 @@ __device__ __forceinline__ size_t t_idx(const Ctx &x, int s, int grp, int k, int
 __global__ void __launch_bounds__(256) k_products(Ctx x) {
 	const Cfg &g = x.cfg;
 	const int K = g.K, LT = g.L, D = LT + 1;
-	const int k0 = blockIdx.x * 32, grp = blockIdx.y, s = x.sBase + blockIdx.z;
+	const int k0 = blockIdx.x * 32, grp = blockIdx.y, s = stream_at(x, x.sBase + blockIdx.z);
 	const int i = threadIdx.x & 31, w = threadIdx.x >> 5;
 	const Call cl = x.call[s];
 	const int base = 32 * grp, nAct = min(32, cl.nFrames - base);
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(32) k_chain_t(Ctx x) {
 	const Cfg &g = x.cfg;
 	const int K = g.K;
 	const int lane = threadIdx.x & 31;
-	const int s = x.sBase + blockIdx.x;
+	const int s = stream_at(x, x.sBase + blockIdx.x);
 	// plain streams of a mixed call: the direct chain.  (A separate read-only load: testing the field of `cl` below costs the
 	// L = 8 stereo instantiation 60 more bytes of spills.)
 	if (!__ldg(&x.call[s].mapped)) return;

@@ -133,6 +133,7 @@ struct CallDesc {
 	// 0); OUTPUT_SEEK its caller rows from seekSamples on (:181)
 	const float *in;
 	int inChan;
+	int slot; // b200s_run_streams: the stream this entry belongs to (entries are in list order); unused without Ctx::listed
 };
 #define B200S_OPBIT(op) (1 << (op))
 
@@ -196,8 +197,8 @@ struct Ctx {
 	float *tE;
 	float *cS, *cM; // [S][maxFrames][K]: smoothed energy (:816-848) and formant envelope (:986-1007) of every block: k_energy / k_passes -> k_prep
 	float *cPitch; // [S][maxFrames] freqEstimate of every block when formantBaseFreq <= 0 (k_pitch)
-	// sub-batch of streams this launch covers (the batch is processed as a few sub-batches on
-	// prioritised CUDA streams so that different kernels of the sequence overlap on the SMs)
+	// sub-batch of streams this launch covers, as positions sBase .. sBase + sCount - 1 (stream_at) (the batch is processed
+	// as a few sub-batches on prioritised CUDA streams so that different kernels of the sequence overlap on the SMs)
 	int sBase, sCount;
 	// I/O of the current call.  nIn / nOut and the rows in / out with their strides are the uniform call's; with `desc` ([S],
 	// b200s_run_per_stream) every stream has its own.  In the process pass only k_plan reads either: it resolves them into
@@ -205,14 +206,20 @@ struct Ctx {
 	// absent from the process pass.  The phase kernels (k_reset_stft, k_reset_bands, k_seek, k_flush_tail, k_add_output)
 	// take, with `desc`, only the streams whose op is in `opMask`, and in / out here are the caller's rows.
 	// outTail > 0 (per-stream calls): output samples from Call::nOut up to outTail are written as zero.
+	// listed (b200s_run_streams): the launch runs over the positions of a list of streams, not over the batch.  Position i
+	// is stream desc[i].slot (stream_at); the caller's I/O rows and desc are indexed by position, state and scratch by stream.
 	const float *in;
 	float *out;
 	int nIn, nOut;
 	const CallDesc *desc;
 	int pass, opMask;
 	int outTail;
+	int listed;
 	long long inStreamStride, outStreamStride; // floats between streams
 	int inChanStride, outChanStride;           // floats between channels
 };
+
+// the stream at position i of a launch (sBase + blockIdx, or a persistent kernel's item): the list's entry, or i itself
+__device__ __forceinline__ int stream_at(const Ctx &x, int i) { return x.listed ? x.desc[i].slot : i; }
 
 } // namespace b200s

@@ -101,6 +101,8 @@ struct b200s_engine {
 	cudaEvent_t evBegin = 0, evSubDone[kMaxSub] = {};
 	int chainedGroups = 0; // > 0: the last operation was a host-buffer process() over this many stream groups (see process_impl)
 	int chainedIn = -1, chainedOut = -1; // its per-channel sample counts (strides): the groups' slabs of the staging buffers sit at sBase*C*n
+	bool chainedListed = false;          // it ran over a list of streams (b200s_run_streams), chainedList, in that order
+	std::vector<int> chainedList;
 	// per-stream call descriptors (b200s_run_per_stream): the device table Ctx::desc [S], allocated at configure, and two
 	// pinned staging copies.  In a call of PROCESS / SKIP ops each stream group copies its own slice on its own CUDA stream
 	// ahead of its k_plan, so chained calls need no join for it; a call with a pre or post phase copies the whole table on
@@ -343,7 +345,8 @@ static int analyse_probe() {
 	return probe;
 }
 #endif
-// mixed: a stereo call with interleaved rows for its plain streams and planar rows for its mapped ones (§3.9 of DESIGN.md)
+// mixed: a stereo call with interleaved rows for its plain streams and planar rows for its mapped ones (§3.9 of DESIGN.md),
+// or a call over a list of streams (§3.13)
 static ChainKernel analyse2_kernel(const Cfg &g, bool mixed = false) {
 	if (mixed) return g.K == 3072 ? k_analyse2_mixed<3072> : k_analyse2_mixed<2560>;
 #ifdef B200S_ANALYSE_PROBES
@@ -987,16 +990,20 @@ static int ensure_buf(b200s_engine *e, float **p, size_t *cap, size_t n, bool ze
 // up to outTail; every other stream is absent from the pass (but for zeros up to outTail in its row).  nIn / nOut are then
 // the rows' strides.  descSlot >= 0: the stream groups upload their slices of the table from pinDesc[descSlot]; -1: the
 // caller has uploaded the whole table on the main stream.  Without desc every stream reads nIn and writes nOut.
+// list (b200s_run_streams, with desc): the call runs over the nList streams list[0..nList), in that order: the rows, the
+// descriptors, the grids and the stream groups are over list positions, and every stream not listed is absent.
 static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, long long inStreamStride, int nIn,
                         float *dOut, int outChanStride, long long outStreamStride, int nOut,
                         const float *hIn = nullptr, float *hOut = nullptr, const short *hIn16 = nullptr, short *hOut16 = nullptr,
-                        const CallDesc *desc = nullptr, int pass = 0, int descSlot = -1, int outTail = 0) {
+                        const CallDesc *desc = nullptr, int pass = 0, int descSlot = -1, int outTail = 0,
+                        const int *list = nullptr, int nList = 0) {
 	const Cfg &g = e->cfg;
 	if (nIn < 0 || nOut < 0) {
 		e->err = "process: negative sample count";
 		return B200S_EINVAL;
 	}
 	const bool perStream = desc != nullptr;
+	const int P = list ? nList : g.S; // positions of the call
 	// the host's decisions over the streams' counts: the longest output sizes the scratch and the grids; a call may need the
 	// random path when ANY stream may stretch beyond 2x; bulk-copy staging needs every input length a multiple of 4
 	int maxOut = nOut;
@@ -1004,14 +1011,15 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	if (perStream) {
 		maxOut = 0;
 		lowRatio = false;
-		for (int s = 0; s < g.S; ++s) {
-			const bool in = desc[s].pass == pass;
-			const int li = in ? desc[s].nIn : 0, lo = in ? desc[s].nOut : 0;
+		anyIdle = P < g.S; // (the streams a list leaves out are absent)
+		for (int i = 0; i < P; ++i) {
+			const bool in = desc[i].pass == pass;
+			const int li = in ? desc[i].nIn : 0, lo = in ? desc[i].nOut : 0;
 			maxOut = std::max(maxOut, lo);
 			if (lo > 0) lowRatio = lowRatio || (long long)li * 2 * g.H < (long long)lo * (g.H + 4);
 			else anyIdle = true;
 			// (an output seek's rows start at its seek window's end: bulk copies need it 16-byte aligned too)
-			lensAligned = lensAligned && li % 4 == 0 && (!in || ((uintptr_t)desc[s].in % 16 == 0 && desc[s].inChan % 4 == 0));
+			lensAligned = lensAligned && li % 4 == 0 && (!in || ((uintptr_t)desc[i].in % 16 == 0 && desc[i].inChan % 4 == 0));
 		}
 	}
 	int rc;
@@ -1059,6 +1067,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 		x.desc = e->dDesc;
 		x.pass = pass;
 		x.outTail = outTail;
+		x.listed = list ? 1 : 0;
 	}
 	// Sub-batch pipeline: the streams of the batch are independent, so the launch sequence is issued
 	// per sub-batch on its own CUDA stream (descending priority).  Sub-batch 0's chain then runs while
@@ -1068,7 +1077,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	const bool hostIO = hIn || hOut || hIn16 || hOut16;
 	const int wantSub = hostIO ? e->nHostParts : e->nSub;
 	// (host-buffer pipeline: at least two streams per group; device-resident sub-batches: only for large batches)
-	const int nSub = (e->profiling || wantSub <= 1 || g.S < (hostIO ? 2 * wantSub : 64)) ? 1 : std::min(wantSub, e->maxSub);
+	const int nSub = (e->profiling || wantSub <= 1 || P < (hostIO ? 2 * wantSub : 64)) ? 1 : std::min(wantSub, e->maxSub);
 	// Consecutive host-buffer calls over the SAME stream groups need no join between them: every group's copies and
 	// kernels are ordered on the group's own stream and touch only that group's streams of the state, so group g of
 	// call n+1 may start its H2D copy while other groups still finish call n (b200s_process_async pipelines calls this
@@ -1077,11 +1086,17 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	// call when the sample counts (the strides of a per-stream call; its streams' own counts may differ) do: a call with
 	// different counts must first join (otherwise group g's copy of call n+1
 	// could overwrite the slab a neighbouring group still uses for call n); evBegin below is that join, since the main
-	// stream has waited for every group's evSubDone at the end of the previous call.
-	const bool chained = hostIO && nSub > 1 && e->chainedGroups == nSub && e->chainedIn == nIn && e->chainedOut == nOut;
+	// stream has waited for every group's evSubDone at the end of the previous call.  A listed call's groups own the streams
+	// at their list positions, so it only chains onto a call over the same list, the same streams in the same order
+	// (otherwise a stream could move to another group and run beside itself).
+	const bool sameStreams = list ? e->chainedListed && (int)e->chainedList.size() == P && std::equal(list, list + P, e->chainedList.begin())
+	                              : !e->chainedListed;
+	const bool chained = hostIO && nSub > 1 && e->chainedGroups == nSub && e->chainedIn == nIn && e->chainedOut == nOut && sameStreams;
 	e->chainedGroups = (hostIO && nSub > 1) ? nSub : 0;
 	e->chainedIn = nIn;
 	e->chainedOut = nOut;
+	e->chainedListed = list != nullptr;
+	if (list) e->chainedList.assign(list, list + P);
 	if (nSub > 1 && !chained) CK(cudaEventRecord(e->evBegin, e->stream));
 	const int chainV = chain_version(g, e->chainV, e->fftV1);
 	const bool pairFft = use_pair_fft(g, e->fftV1);
@@ -1089,8 +1104,8 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 	for (int sub = 0; sub < nSub; ++sub) {
 		cudaStream_t st = nSub > 1 ? e->subStream[sub] : e->stream;
 		if (nSub > 1 && !chained) CK(cudaStreamWaitEvent(st, e->evBegin, 0));
-		x.sBase = (int)((long long)g.S * sub / nSub);
-		x.sCount = (int)((long long)g.S * (sub + 1) / nSub) - x.sBase;
+		x.sBase = (int)((long long)P * sub / nSub);
+		x.sCount = (int)((long long)P * (sub + 1) / nSub) - x.sBase;
 		if (perStream && descSlot >= 0) { // the group's slice of the table, ordered before its k_plan and after its previous call's kernels
 			CK(cudaMemcpyAsync(e->dDesc + x.sBase, e->pinDesc[descSlot] + x.sBase, sizeof(CallDesc) * x.sCount, cudaMemcpyHostToDevice, st));
 			CK(cudaEventRecord(e->evDesc[descSlot][sub], st));
@@ -1109,7 +1124,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 				if (pairFft) { // persistent CTAs, two per SM, over the (stream, job pair) items
 					const long long items = (long long)x.sCount * g.C * x.maxFrames;
 					const int grid = (int)std::min<long long>(items, 2LL * e->numSMs);
-					PROF(PK_ANALYSE, B200S_LAUNCH(analyse2_kernel(g, x.specIl && anyMapped), dim3(grid), dim3(256), smem_analyse2(g), st, x));
+					PROF(PK_ANALYSE, B200S_LAUNCH(analyse2_kernel(g, (x.specIl && anyMapped) || x.listed), dim3(grid), dim3(256), smem_analyse2(g), st, x));
 				} else {
 					ChainKernel ka = analyse_kernel(g);
 					PROF(PK_ANALYSE, B200S_LAUNCH(ka, dim3(std::min(2 * F * g.C, ANALYSE_CTAS_PER_STREAM), 1, x.sCount), dim3(kThreads), smem_analyse(g), st, x));
@@ -1252,7 +1267,7 @@ static int process_impl(b200s_engine *e, const float *dIn, int inChanStride, lon
 			CK(cudaStreamWaitEvent(e->stream, e->evSubDone[sub], 0));
 		}
 	}
-	e->histCur ^= 1;
+	if (!list) e->histCur ^= 1; // (a listed call's k_commit copies the new history back into histCur)
 	return 0;
 }
 
@@ -1356,17 +1371,21 @@ static int fetch_out(b200s_engine *e, float *out, int n) {
 // unchanged into the other buffer.  A phase that no stream needs is not launched.  Host buffers: a call of PROCESS / SKIP
 // ops with some PROCESS pipelines its stream groups as b200s_process_async does; any other call copies the input slab in
 // on the main stream, runs on the device and copies the output slab back.
+// list (b200s_run_streams): the call runs over the n streams list[0..n) instead of the batch.  The arrays, the rows and the
+// descriptor table are over list positions i (stream list[i]), and so are the grids of every phase; the streams not listed
+// are not part of the call at all.
 static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStride, const int *nIn, float *out, int outStride,
-                    const int *nOut, const double *rates, bool host, bool wait) {
+                    const int *nOut, const double *rates, bool host, bool wait, const int *list = nullptr, int n = 0) {
 	const Cfg &g = e->cfg;
 	const long long C = g.C;
 	const int inLat = g.B - g.B / 2, outLat = g.B / 2 + (g.split ? g.H : 0);
+	const int P = list ? n : g.S; // positions of the call
 	int opsUsed = 0, zeroLen = 0;
-	for (int s = 0; s < g.S; ++s) {
-		opsUsed |= B200S_OPBIT(ops[s]);
-		if (ops[s] == B200S_OP_FLUSH) {
-			const int outputBlock = std::max(0, nOut[s] - g.H); // :439
-			zeroLen = std::max(zeroLen, std::max(0, int(outputBlock * (rates ? float(rates[s]) : 0.f)))); // :440
+	for (int i = 0; i < P; ++i) {
+		opsUsed |= B200S_OPBIT(ops[i]);
+		if (ops[i] == B200S_OP_FLUSH) {
+			const int outputBlock = std::max(0, nOut[i] - g.H); // :439
+			zeroLen = std::max(zeroLen, std::max(0, int(outputBlock * (rates ? float(rates[i]) : 0.f)))); // :440
 		}
 	}
 	const int preOps = B200S_OPBIT(B200S_OP_RESET) | B200S_OPBIT(B200S_OP_SEEK) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
@@ -1385,19 +1404,20 @@ static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStri
 	// (sized by b200s_reserve: no allocation then)
 	if ((opsUsed & B200S_OPBIT(B200S_OP_FLUSH)) && (rc = ensure_buf(e, &e->dZero, &e->zeroCap, (size_t)std::max(zeroLen, 1), true))) return rc;
 	// An output seek writes outputLatency samples of pre-roll into its output rows, which k_add_output reads back and then
-	// zeroes.  Rows narrower than that: the pass writes into dTmp [S][C][outputLatency], copied back to the caller's rows.
+	// zeroes.  Rows narrower than that: the pass writes into dTmp [positions][C][outputLatency], copied back to the caller's rows.
 	const int W = (opsUsed & B200S_OPBIT(B200S_OP_OUTPUT_SEEK)) ? std::max(outStride, outLat) : outStride;
-	if (W > outStride && (rc = ensure_buf(e, &e->dTmp, &e->tmpCap, (size_t)g.S * C * W, false))) return rc;
+	if (W > outStride && (rc = ensure_buf(e, &e->dTmp, &e->tmpCap, (size_t)P * C * W, false))) return rc;
 	const float *dIn = host ? e->dIn : in;
 	float *dOut = host ? e->dOut : out, *pOut = W > outStride ? e->dTmp : dOut;
 	const int lk = e->descSlot ^= 1;
 	for (int i = 0; i < b200s_engine::kMaxSub; ++i) CK(cudaEventSynchronize(e->evDesc[lk][i]));
 	CallDesc *d = e->pinDesc[lk];
 	bool anyPass = false, seekSlow = false;
-	for (int s = 0; s < g.S; ++s) {
+	for (int s = 0; s < P; ++s) { // (s: the position)
 		CallDesc c;
 		memset(&c, 0, sizeof(c));
 		c.op = ops[s];
+		c.slot = list ? list[s] : s;
 		c.in = dIn + (size_t)s * C * inStride;
 		c.inChan = inStride;
 		switch (c.op) {
@@ -1442,59 +1462,61 @@ static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStri
 		d[s] = c;
 	}
 	if (host && !phases && anyPass) { // the stream groups copy their own slabs in and out
-		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, d, 1, lk, outStride))) return rc;
+		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, d, 1, lk, outStride, list, n))) return rc;
 		if (wait) CK(cudaStreamSynchronize(e->stream));
 		return 0;
 	}
 	if (host) {
 		e->chainedGroups = 0;
-		if (in && inStride > 0) CK(cudaMemcpyAsync(e->dIn, in, sizeof(float) * (size_t)g.S * C * inStride, cudaMemcpyHostToDevice, e->stream));
+		if (in && inStride > 0) CK(cudaMemcpyAsync(e->dIn, in, sizeof(float) * (size_t)P * C * inStride, cudaMemcpyHostToDevice, e->stream));
 	}
 	if (phases) { // the whole table on the main stream, ahead of the pre phase (the call joins)
 		e->chainedGroups = 0;
-		CK(cudaMemcpyAsync(e->dDesc, d, sizeof(CallDesc) * g.S, cudaMemcpyHostToDevice, e->stream));
+		CK(cudaMemcpyAsync(e->dDesc, d, sizeof(CallDesc) * P, cudaMemcpyHostToDevice, e->stream));
 		CK(cudaEventRecord(e->evDesc[lk][0], e->stream));
 	}
 	Ctx x = make_ctx(e);
 	x.desc = e->dDesc;
+	x.listed = list ? 1 : 0;
 	x.in = dIn; x.inChanStride = inStride; x.inStreamStride = C * inStride;
 	if (opsUsed & preOps) {
 		if (opsUsed & (B200S_OPBIT(B200S_OP_RESET) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK))) {
 			x.opMask = B200S_OPBIT(B200S_OP_RESET) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
-			PROF(PK_PHASE, B200S_LAUNCH(k_reset_stft, dim3(g.S), dim3(kThreads), 0, e->stream, x));
-			PROF(PK_PHASE, B200S_LAUNCH(k_reset_bands, dim3(g.S), dim3(kThreads), 0, e->stream, x, 15));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_stft, dim3(P), dim3(kThreads), 0, e->stream, x));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_bands, dim3(P), dim3(kThreads), 0, e->stream, x, 15));
 		}
 		if (opsUsed & (B200S_OPBIT(B200S_OP_SEEK) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK))) {
 			x.opMask = B200S_OPBIT(B200S_OP_SEEK) | B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
-			PROF(PK_PHASE, B200S_LAUNCH(k_seek, dim3(g.S), dim3(kThreads), 0, e->stream, x, 0.f));
+			PROF(PK_PHASE, B200S_LAUNCH(k_seek, dim3(P), dim3(kThreads), 0, e->stream, x, 0.f));
 			e->seekMayRandom = e->seekMayRandom || seekSlow; // (other streams may still carry an earlier seek's factor)
 		}
 	}
 	if (anyPass) {
-		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, pOut, W, C * W, W, nullptr, nullptr, nullptr, nullptr, d, 1, phases ? -1 : lk, W))) return rc;
+		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, pOut, W, C * W, W, nullptr, nullptr, nullptr, nullptr, d, 1, phases ? -1 : lk, W, list, n))) return rc;
 	} else if (W > 0) { // no process pass: every row is zero but for the flushes' tails (post phase)
-		const size_t cnt = (size_t)g.S * C * W;
+		const size_t cnt = (size_t)P * C * W;
 		PROF(PK_PHASE, B200S_LAUNCH(k_zero, dim3((unsigned)std::min<size_t>((cnt + 1023) / 1024, 4096)), dim3(256), 0, e->stream, pOut, cnt));
 	}
 	if (opsUsed & postOps) {
-		Ctx y = make_ctx(e); // (after the pass's history flip)
+		Ctx y = make_ctx(e); // (after the pass: the history buffer it left current)
 		y.desc = e->dDesc;
+		y.listed = x.listed;
 		y.out = pOut; y.outChanStride = W; y.outStreamStride = C * W;
 		y.outTail = W;
 		if (opsUsed & B200S_OPBIT(B200S_OP_FLUSH)) {
 			y.opMask = B200S_OPBIT(B200S_OP_FLUSH);
-			PROF(PK_PHASE, B200S_LAUNCH(k_flush_tail, dim3(g.C, g.S), dim3(kThreads), sizeof(float) * g.B, e->stream, y, 0, 0));
-			PROF(PK_PHASE, B200S_LAUNCH(k_reset_stft, dim3(g.S), dim3(kThreads), 0, e->stream, y));
-			PROF(PK_PHASE, B200S_LAUNCH(k_reset_bands, dim3(g.S), dim3(kThreads), 0, e->stream, y, 6));
+			PROF(PK_PHASE, B200S_LAUNCH(k_flush_tail, dim3(g.C, P), dim3(kThreads), sizeof(float) * g.B, e->stream, y, 0, 0));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_stft, dim3(P), dim3(kThreads), 0, e->stream, y));
+			PROF(PK_PHASE, B200S_LAUNCH(k_reset_bands, dim3(P), dim3(kThreads), 0, e->stream, y, 6));
 		}
 		if (opsUsed & B200S_OPBIT(B200S_OP_OUTPUT_SEEK)) {
 			y.opMask = B200S_OPBIT(B200S_OP_OUTPUT_SEEK);
-			PROF(PK_PHASE, B200S_LAUNCH(k_add_output, dim3(g.C, g.S), dim3(kThreads), 0, e->stream, y, (const float *)nullptr, outLat));
+			PROF(PK_PHASE, B200S_LAUNCH(k_add_output, dim3(g.C, P), dim3(kThreads), 0, e->stream, y, (const float *)nullptr, outLat));
 		}
 	}
 	if (pOut != dOut && outStride > 0)
-		PROF(PK_PHASE, B200S_LAUNCH(k_copy_rows, dim3((unsigned)std::min<long long>((long long)g.S * C, 65535)), dim3(256), 0, e->stream, dOut, outStride, (const float *)pOut, W, outStride, (int)(g.S * C)));
-	if (host && out && outStride > 0) CK(cudaMemcpyAsync(out, e->dOut, sizeof(float) * (size_t)g.S * C * outStride, cudaMemcpyDeviceToHost, e->stream));
+		PROF(PK_PHASE, B200S_LAUNCH(k_copy_rows, dim3((unsigned)std::min<long long>((long long)P * C, 65535)), dim3(256), 0, e->stream, dOut, outStride, (const float *)pOut, W, outStride, (int)(P * C)));
+	if (host && out && outStride > 0) CK(cudaMemcpyAsync(out, e->dOut, sizeof(float) * (size_t)P * C * outStride, cudaMemcpyDeviceToHost, e->stream));
 	if (wait) CK(cudaStreamSynchronize(e->stream));
 	return 0;
 }
@@ -2130,9 +2152,12 @@ int b200s_process_async(b200s_engine *e, const float *in, int nIn, float *out, i
 	if ((rc = stage_out(e, nOut))) return rc;
 	return process_impl(e, e->dIn, nIn, (long long)e->cfg.C * nIn, nIn, e->dOut, nOut, (long long)e->cfg.C * nOut, nOut, in, out);
 }
-// Arguments of the per-stream calls, checked before anything is enqueued
-static int check_run(b200s_engine *e, const char *fn, const int *ops, int inStride, const int *nIn, int outStride, const int *nOut, const double *rates) {
-	if (!ops || !nIn || !nOut) {
+// Arguments of the per-stream calls, checked before anything is enqueued: the batch's S entries, or the n entries of a
+// list (the message then names the entry and its stream)
+static int check_run(b200s_engine *e, const char *fn, const int *ops, int inStride, const int *nIn, int outStride, const int *nOut, const double *rates,
+                     const int *list = nullptr, int n = -1) {
+	const int P = n >= 0 ? n : e->S;
+	if (P > 0 && (!ops || !nIn || !nOut)) {
 		e->err = std::string(fn) + ": " + (ops ? "input_samples and output_samples must not be NULL" : "ops must not be NULL");
 		return B200S_EINVAL;
 	}
@@ -2140,7 +2165,7 @@ static int check_run(b200s_engine *e, const char *fn, const int *ops, int inStri
 		e->err = std::string(fn) + ": negative stride";
 		return B200S_EINVAL;
 	}
-	for (int s = 0; s < e->S; ++s) {
+	for (int s = 0; s < P; ++s) {
 		const int op = ops[s];
 		std::string why;
 		if (op < B200S_OP_SKIP || op > B200S_OP_RESET) why = "op " + std::to_string(op) + " is not a B200S_OP_*";
@@ -2154,7 +2179,7 @@ static int check_run(b200s_engine *e, const char *fn, const int *ops, int inStri
 		else if (nOut[s] < 0 || nOut[s] > outStride)
 			why = "output_samples " + std::to_string(nOut[s]) + " is outside [0, " + std::to_string(outStride) + "]";
 		if (!why.empty()) {
-			e->err = std::string(fn) + ": stream " + std::to_string(s) + ": " + why;
+			e->err = std::string(fn) + ": " + (list ? "entry " + std::to_string(s) + " (stream " + std::to_string(list[s]) + ")" : "stream " + std::to_string(s)) + ": " + why;
 			return B200S_EINVAL;
 		}
 	}
@@ -2178,6 +2203,32 @@ int b200s_run_per_stream_async(b200s_engine *e, const int *ops, const float *in,
 int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *dIn, int inStride, const int *nIn, float *dOut, int outStride,
                                 const int *nOut, const double *rates) {
 	return run_entry(e, "b200s_run_per_stream_device", ops, dIn, inStride, nIn, dOut, outStride, nOut, rates, false, false);
+}
+// b200s_run_per_stream over a list of streams
+static int run_streams_entry(b200s_engine *e, const char *fn, int n, const int *streams, const int *ops, const float *in, int inStride,
+                             const int *nIn, float *out, int outStride, const int *nOut, const double *rates, bool host, bool wait) {
+	NEED_CFG();
+	if (n < 0 || n > e->S) {
+		e->err = std::string(fn) + ": n = " + std::to_string(n) + " is outside [0, " + std::to_string(e->S) + "]";
+		return B200S_EINVAL;
+	}
+	if (!check_streams(e->err, fn, "streams", streams, n, e->S, true)) return B200S_EINVAL;
+	int rc;
+	if ((rc = check_run(e, fn, ops, inStride, nIn, outStride, nOut, rates, streams, n))) return rc;
+	if (n == 0) return 0;
+	return run_impl(e, ops, in, inStride, nIn, out, outStride, nOut, rates, host, wait, streams, n);
+}
+int b200s_run_streams(b200s_engine *e, int n, const int *streams, const int *ops, const float *in, int inStride, const int *nIn,
+                      float *out, int outStride, const int *nOut, const double *rates) {
+	return run_streams_entry(e, "b200s_run_streams", n, streams, ops, in, inStride, nIn, out, outStride, nOut, rates, true, true);
+}
+int b200s_run_streams_async(b200s_engine *e, int n, const int *streams, const int *ops, const float *in, int inStride, const int *nIn,
+                            float *out, int outStride, const int *nOut, const double *rates) {
+	return run_streams_entry(e, "b200s_run_streams_async", n, streams, ops, in, inStride, nIn, out, outStride, nOut, rates, true, false);
+}
+int b200s_run_streams_device(b200s_engine *e, int n, const int *streams, const int *ops, const float *dIn, int inStride, const int *nIn,
+                             float *dOut, int outStride, const int *nOut, const double *rates) {
+	return run_streams_entry(e, "b200s_run_streams_device", n, streams, ops, dIn, inStride, nIn, dOut, outStride, nOut, rates, false, false);
 }
 // process() with per-stream lengths: b200s_run_per_stream with every op PROCESS
 int b200s_process_per_stream(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {

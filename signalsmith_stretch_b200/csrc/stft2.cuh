@@ -40,7 +40,8 @@ __device__ __forceinline__ void st_stream(float *p, float v) { __stcs(p, v); }
 // 3 the wait for the staged input (moved to just before the next copies are issued), 4 the FFT's stages B and C.
 // ---------------------------------------------------------------------------------------------
 // MIXED (k_analyse2_mixed): a stereo call whose streams take both paths -- the store form is chosen per item, planar
-// rows for the streams on the mapped path (spec_il).  Otherwise (k_analyse2) the form is the call's, x.specIl, and the
+// rows for the streams on the mapped path (spec_il) -- and every call over a list of streams (Ctx::listed: the item's
+// stream is looked up in the list; k_analyse2 keeps the whole batch's item fetch, which is on its critical path).  Otherwise (k_analyse2) the form is the call's, x.specIl, and the
 // per-item test is not in the code at all.
 template <int KT, int PROBE, bool MIXED>
 __device__ __forceinline__ void analyse2_body(const Ctx &x) {
@@ -66,8 +67,15 @@ __device__ __forceinline__ void analyse2_body(const Ctx &x) {
 	// fetch_raw only issues the loads (m.hasB temporarily holds the stream's job count); fetch_done turns them into
 	// an item.  Keeping the two apart lets the loads of the item after next fly for a whole iteration.
 	auto fetch_raw = [&](long long it, Item &m) {
-		m.s = x.sBase + (int)(it / PJ);
-		const Job *jb = x.jobs + (size_t)m.s * 2 * g.C * x.maxFrames + 2 * (int)(it % PJ);
+		const Job *jb;
+		if constexpr (MIXED) { // (one 64-bit division, not two: with the list look-up the kernel fits 128 registers)
+			const int q = (int)(it / PJ);
+			m.s = stream_at(x, x.sBase + q);
+			jb = x.jobs + (size_t)m.s * 2 * g.C * x.maxFrames + 2 * (int)(it - (long long)q * PJ);
+		} else {
+			m.s = x.sBase + (int)(it / PJ);
+			jb = x.jobs + (size_t)m.s * 2 * g.C * x.maxFrames + 2 * (int)(it % PJ);
+		}
 		m.hasB = x.call[m.s].nJobs;
 		m.nIn = x.call[m.s].nIn;
 		m.in = x.call[m.s].in;
@@ -318,9 +326,9 @@ __device__ __forceinline__ void synth2_body(const Ctx &x) {
 	B200S_DYN_SHARED
 	float4 *buf = (float4 *)dyn_smem;
 	float *pend = (float *)(buf + G::LEN);
-	const int c = blockIdx.x, s = x.sBase + blockIdx.y, tid = threadIdx.x;
+	const int c = blockIdx.x, pos = x.sBase + blockIdx.y, s = stream_at(x, pos), tid = threadIdx.x;
 	const Call cl = x.call[s];
-	float *out = x.out + (size_t)s * x.outStreamStride + (size_t)c * x.outChanStride;
+	float *out = x.out + (size_t)pos * x.outStreamStride + (size_t)c * x.outChanStride; // (the caller's row: by position)
 	if (cl.bypass) { // :252-267
 		const float *in = cl.in + (size_t)c * cl.inChan;
 		for (int i = tid; i < cl.nOut; i += 256) out[i] = cl.nIn > 0 ? in[i % cl.nIn] : 0.f;
