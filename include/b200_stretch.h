@@ -223,6 +223,27 @@ int b200s_run_streams_async(b200s_engine *e, int n, const int *streams, const in
 int b200s_run_streams_device(b200s_engine *e, int n, const int *streams, const int *ops, const float *d_in, int in_stride,
                              const int *input_samples, float *d_out, int out_stride, const int *output_samples,
                              const double *playback_rates);
+/* b200s_run_per_stream and b200s_run_streams with 16-bit PCM host buffers, [positions][channels][stride] shorts: half the
+ * bytes over PCIe of the float calls.  Per-stream lengths with plain process() are b200s_run_per_stream_pcm16 with every
+ * op B200S_OP_PROCESS.
+ *   - Every output row, state included, is bit-identical to the float call with the same arguments fed in / 32768, its
+ *     output converted as b200s_process_pcm16 converts it: * 32768, round to nearest with halves away from zero, clamp to
+ *     [-32768, 32767].  This holds for every op.  Both conversions run on the device.
+ *   - Every output sample an op does not produce is 0, up to out_stride.  Slots a listed call leaves out are neither read
+ *     nor written.
+ *   - B200S_EINVAL, before anything is enqueued and with the same messages: every rule of the float counterpart.
+ *   - wait = 0: the call returns once enqueued, like b200s_run_per_stream_async / b200s_run_streams_async.  A call of
+ *     PROCESS / SKIP ops pipelines by the float calls' rule (the same list in the same order, the same strides; the sample
+ *     format does not matter); any other call joins.  `in` must stay valid and `out` must not be read until
+ *     b200s_synchronize(); pinned host memory is needed for the copies to be asynchronous.
+ *   - The 16-bit staging of b200s_process_pcm16, [positions][channels][stride] each way, grows on first use after a
+ *     synchronisation of the handle's stream; a later call at no larger strides and positions allocates nothing.
+ *     b200s_reserve does not size it. */
+int b200s_run_per_stream_pcm16(b200s_engine *e, const int *ops, const short *in, int in_stride, const int *input_samples,
+                               short *out, int out_stride, const int *output_samples, const double *playback_rates, int wait);
+int b200s_run_streams_pcm16(b200s_engine *e, int n, const int *streams, const int *ops, const short *in, int in_stride,
+                            const int *input_samples, short *out, int out_stride, const int *output_samples,
+                            const double *playback_rates, int wait);
 
 /* ---- moving, duplicating and saving single streams ----
  * A server that rebalances streams over engines or GPUs, forks a session to preview two settings from the same point,

@@ -35,6 +35,7 @@ ABI_SYMBOLS = [
     "b200s_process_per_stream", "b200s_process_per_stream_async", "b200s_process_per_stream_device",
     "b200s_run_per_stream", "b200s_run_per_stream_async", "b200s_run_per_stream_device",
     "b200s_run_streams", "b200s_run_streams_async", "b200s_run_streams_device",
+    "b200s_run_per_stream_pcm16", "b200s_run_streams_pcm16",
     "b200s_timer_start", "b200s_timer_stop", "b200s_kernel_launches", "b200s_device_allocations", "b200s_unserved_random_blocks", "b200s_profile_begin", "b200s_profile_end",
     "b200s_selftest_divsqrt",
     "b200s_state_size", "b200s_get_state", "b200s_set_state",
@@ -111,6 +112,8 @@ def _bind(lib):
         "b200s_run_streams": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
         "b200s_run_streams_async": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
         "b200s_run_streams_device": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd)]),
+        "b200s_run_per_stream_pcm16": (ci, [vp, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd), ci]),
+        "b200s_run_streams_pcm16": (ci, [vp, ci, ip, ip, vp, ci, ip, vp, ci, ip, ctypes.POINTER(cd), ci]),
         "b200s_timer_start": (ci, [vp]), "b200s_timer_stop": (ci, [vp, fp]), "b200s_kernel_launches": (cll, [vp]), "b200s_device_allocations": (cll, [vp]), "b200s_unserved_random_blocks": (cll, [vp]),
         "b200s_profile_begin": (ci, [vp]), "b200s_profile_end": (ci, [vp, fp, ip, ci]),
         "b200s_selftest_divsqrt": (ci, [vp, cll, cll, ctypes.POINTER(cll), ctypes.POINTER(cll)]),
@@ -410,25 +413,14 @@ class BatchStretch:
         self._ck(self._lib.b200s_process(self._h, x.ctypes.data, n_in, out.ctypes.data, outputSamples))
         return out
 
-    def run(self, ops, inputs, outputSamples, inputSamples=None, playbackRates=None, out=None, streams=None):
-        """Every stream runs its own operation (b200s_run_per_stream): ops, outputSamples, inputSamples and playbackRates are
-        scalars (repeated for every stream) or one value per stream.  OP_PROCESS: process(inputs[s][:, :inputSamples[s]],
-        outputSamples[s]); OP_SEEK: seek(inputs[s][:, :inputSamples[s]], playbackRates[s]); OP_OUTPUT_SEEK:
-        outputSeek(inputs[s][:, :inputSamples[s]]); OP_FLUSH: flush(outputSamples[s], playbackRates[s]); OP_RESET: reset();
-        OP_SKIP: nothing.  inputs: [batch][channels][stride] (numpy -> host API; torch CUDA tensor -> device API; None
-        when no stream reads input); inputSamples defaults to the whole stride for the ops that read input and 0 for the
-        others.  Returns [batch][channels][max(outputSamples)] (or `out`), zeros after each stream's own output.
-
-        streams: a list of n slots (b200s_run_streams).  Only they run; every array then has one value per list entry and
-        the buffers are [n][channels][stride], row i for stream streams[i].  The other streams are not touched."""
-        torch_in = _is_torch_cuda(inputs)
+    def _run_args(self, ops, in_stride, outputSamples, inputSamples, playbackRates, out, streams):
+        """The checked arguments of run() / run_pcm16(): (rows, list or None, ops, n_in, n_out, rates or None, out_stride)."""
         lst = None if streams is None else self._stream_list(streams, "streams")
         rows = self.batch if lst is None else int(lst.size)
         op = self._lengths(ops, "ops", rows)
         if np.any((op < 0) | (op > 5)):
             raise ValueError("ops: every op must be one of OP_SKIP .. OP_RESET")
         n_out = self._lengths(outputSamples, "outputSamples", rows)
-        in_stride = 0 if inputs is None else int(inputs.shape[-1]) if torch_in else int(np.shape(inputs)[-1])
         if inputSamples is None:
             reads = (op == self.OP_PROCESS) | (op == self.OP_SEEK) | (op == self.OP_OUTPUT_SEEK)
             inputSamples = np.where(reads, in_stride, 0)
@@ -448,12 +440,31 @@ class BatchStretch:
             bad = np.flatnonzero((a < 0) | (a > stride))
             if bad.size:
                 raise ValueError("%s[%d] = %d is outside [0, %d]" % (name, bad[0], a[bad[0]], stride))
+        return rows, lst, op, n_in, n_out, rates, out_stride
+
+    def _run_call(self, fn_all, fn_list, lst, op, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, rates, *extra):
         ip, dp = ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_double)
         rp = None if rates is None else rates.ctypes.data_as(dp)
+        args = (op.ctypes.data_as(ip), in_ptr, in_stride, n_in.ctypes.data_as(ip), out_ptr, out_stride, n_out.ctypes.data_as(ip), rp) + extra
+        self._ck(fn_all(self._h, *args) if lst is None else fn_list(self._h, int(lst.size), lst.ctypes.data_as(ip), *args))
+
+    def run(self, ops, inputs, outputSamples, inputSamples=None, playbackRates=None, out=None, streams=None):
+        """Every stream runs its own operation (b200s_run_per_stream): ops, outputSamples, inputSamples and playbackRates are
+        scalars (repeated for every stream) or one value per stream.  OP_PROCESS: process(inputs[s][:, :inputSamples[s]],
+        outputSamples[s]); OP_SEEK: seek(inputs[s][:, :inputSamples[s]], playbackRates[s]); OP_OUTPUT_SEEK:
+        outputSeek(inputs[s][:, :inputSamples[s]]); OP_FLUSH: flush(outputSamples[s], playbackRates[s]); OP_RESET: reset();
+        OP_SKIP: nothing.  inputs: [batch][channels][stride] (numpy -> host API; torch CUDA tensor -> device API; None
+        when no stream reads input); inputSamples defaults to the whole stride for the ops that read input and 0 for the
+        others.  Returns [batch][channels][max(outputSamples)] (or `out`), zeros after each stream's own output.
+
+        streams: a list of n slots (b200s_run_streams).  Only they run; every array then has one value per list entry and
+        the buffers are [n][channels][stride], row i for stream streams[i].  The other streams are not touched."""
+        torch_in = _is_torch_cuda(inputs)
+        in_stride = 0 if inputs is None else int(inputs.shape[-1]) if torch_in else int(np.shape(inputs)[-1])
+        rows, lst, op, n_in, n_out, rates, out_stride = self._run_args(ops, in_stride, outputSamples, inputSamples, playbackRates, out, streams)
 
         def call(fn_all, fn_list, in_ptr, out_ptr):
-            args = (op.ctypes.data_as(ip), in_ptr, in_stride, n_in.ctypes.data_as(ip), out_ptr, out_stride, n_out.ctypes.data_as(ip), rp)
-            self._ck(fn_all(self._h, *args) if lst is None else fn_list(self._h, rows, lst.ctypes.data_as(ip), *args))
+            self._run_call(fn_all, fn_list, lst, op, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, rates)
 
         if torch_in:
             import torch
@@ -475,6 +486,31 @@ class BatchStretch:
         if out is None:
             out = np.empty(self._shape(out_stride, rows), np.float32)
         call(self._lib.b200s_run_per_stream, self._lib.b200s_run_streams, None if x is None else x.ctypes.data, out.ctypes.data)
+        return out
+
+    def run_pcm16(self, ops, inputs, outputSamples, inputSamples=None, playbackRates=None, out=None, streams=None):
+        """run() with 16-bit PCM host buffers (b200s_run_per_stream_pcm16 / b200s_run_streams_pcm16): inputs is an int16
+        array [rows][channels][stride] (or None), the result an int16 array [rows][channels][out_stride] (or `out`).  The
+        output equals run() fed inputs / 32768, rounded to nearest (halves away from zero) and clamped to int16; both
+        conversions run on the device.  There is no device-buffer form: a torch CUDA tensor raises TypeError."""
+        if _is_torch_cuda(inputs) or _is_torch_cuda(out):
+            raise TypeError("run_pcm16: 16-bit PCM is a host-buffer format; pass float32 CUDA tensors to run()")
+        in_stride = 0 if inputs is None else int(np.shape(inputs)[-1])
+        rows, lst, op, n_in, n_out, rates, out_stride = self._run_args(ops, in_stride, outputSamples, inputSamples, playbackRates, out, streams)
+        x = None
+        if inputs is not None:
+            x = np.asarray(inputs)
+            if x.dtype != np.int16:
+                raise ValueError("inputs: expected int16 samples, got %s" % x.dtype)
+            if x.shape != self._shape(in_stride, rows):
+                raise ValueError("inputs: expected shape %s, got %s" % (self._shape(in_stride, rows), x.shape))
+            x = np.ascontiguousarray(x)
+        if out is None:
+            out = np.empty(self._shape(out_stride, rows), np.int16)
+        elif not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.flags.c_contiguous):
+            raise ValueError("out: expected a contiguous int16 numpy array")
+        self._run_call(self._lib.b200s_run_per_stream_pcm16, self._lib.b200s_run_streams_pcm16, lst, op, None if x is None else x.ctypes.data,
+                       in_stride, n_in, out.ctypes.data, out_stride, n_out, rates, 1)
         return out
 
     def process_per_stream_host_ptr(self, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, wait=False):
@@ -509,6 +545,17 @@ class BatchStretch:
         fn = self._lib.b200s_run_streams if wait else self._lib.b200s_run_streams_async
         self._ck(fn(self._h, n, lst.ctypes.data_as(ip), o.ctypes.data_as(ip), in_ptr, int(in_stride), a.ctypes.data_as(ip), out_ptr,
                     int(out_stride), b.ctypes.data_as(ip), rp))
+
+    def run_pcm16_host_ptr(self, ops, in_ptr, in_stride, n_in, out_ptr, out_stride, n_out, playback_rates=None, streams=None, wait=False):
+        """Raw host pointers to pinned int16 buffers [rows][channels][stride]: b200s_run_per_stream_pcm16, or with `streams`
+        b200s_run_streams_pcm16 (rows = len(streams)).  Unless `wait` the call returns once enqueued and the buffers belong
+        to the engine until synchronize(); ops, counts and rates are copied during the call."""
+        lst = None if streams is None else self._stream_list(streams, "streams")
+        rows = self.batch if lst is None else int(lst.size)
+        o, a, b = self._lengths(ops, "ops", rows), self._lengths(n_in, "n_in", rows), self._lengths(n_out, "n_out", rows)
+        r = None if playback_rates is None else np.ascontiguousarray(np.broadcast_to(np.asarray(playback_rates, np.float64), (rows,)))
+        self._run_call(self._lib.b200s_run_per_stream_pcm16, self._lib.b200s_run_streams_pcm16, lst, o, in_ptr, int(in_stride), a, out_ptr,
+                       int(out_stride), b, r, 1 if wait else 0)
 
     def process_host_ptr(self, in_ptr, n_in, out_ptr, n_out):
         """Raw host pointers (e.g. pinned torch tensors): the end-to-end call bench.py times."""

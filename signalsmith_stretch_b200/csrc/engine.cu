@@ -172,7 +172,7 @@ struct b200s_engine {
 	// staging for the host-buffer API and for flush/outputSeek
 	float *dIn = 0, *dOut = 0, *dZero = 0, *dTmp = 0;
 	size_t inCap = 0, outCap = 0, zeroCap = 0, tmpCap = 0;
-	short *dIn16 = 0, *dOut16 = 0; // 16-bit PCM staging of b200s_process_pcm16
+	short *dIn16 = 0, *dOut16 = 0; // 16-bit PCM staging of b200s_process_pcm16 and the _pcm16 per-stream calls (stage_pcm16)
 	size_t in16Cap = 0, out16Cap = 0;
 	// stream copies, export and import (DESIGN.md §3.12): packed records [xferCap][record bytes], the stream lists of the
 	// pack and the unpack (device [2][xferCap]; two pinned staging copies, rewritten once the upload issued from them two
@@ -1355,6 +1355,21 @@ static int stage_out(b200s_engine *e, int n) {
 	size_t cnt = (size_t)e->cfg.S * e->cfg.C * std::max(n, 1);
 	return ensure_buf(e, &e->dOut, &e->outCap, cnt, false);
 }
+// the 16-bit PCM slabs, ci / co samples; growing one first drains the handle's stream (copies may still use the old one)
+static int stage_pcm16(b200s_engine *e, size_t ci, size_t co) {
+	if (ci <= e->in16Cap && co <= e->out16Cap) return 0;
+	CK(cudaStreamSynchronize(e->stream));
+	int rc;
+	if (ci > e->in16Cap) {
+		if ((rc = dalloc(e, &e->dIn16, ci))) return rc;
+		e->in16Cap = ci;
+	}
+	if (co > e->out16Cap) {
+		if ((rc = dalloc(e, &e->dOut16, co))) return rc;
+		e->out16Cap = co;
+	}
+	return 0;
+}
 static int fetch_out(b200s_engine *e, float *out, int n) {
 	if (n > 0) CK(cudaMemcpyAsync(out, e->dOut, sizeof(float) * (size_t)e->cfg.S * e->cfg.C * n, cudaMemcpyDeviceToHost, e->stream));
 	CK(cudaStreamSynchronize(e->stream));
@@ -1374,8 +1389,13 @@ static int fetch_out(b200s_engine *e, float *out, int n) {
 // list (b200s_run_streams): the call runs over the n streams list[0..n) instead of the batch.  The arrays, the rows and the
 // descriptor table are over list positions i (stream list[i]), and so are the grids of every phase; the streams not listed
 // are not part of the call at all.
+// in16 / out16 (the _pcm16 calls, host buffers, `in` / `out` NULL): 16-bit PCM rows [positions][C][stride], copied through
+// the dIn16 / dOut16 slabs and converted to and from the float rows of dIn / dOut on the device.  A joining call converts
+// its input ahead of the pre phase and its output after the post phase and k_copy_rows (the output seeks' pre-roll and the
+// flushes' tails are only final then); a chained call converts per stream group in process_impl.
 static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStride, const int *nIn, float *out, int outStride,
-                    const int *nOut, const double *rates, bool host, bool wait, const int *list = nullptr, int n = 0) {
+                    const int *nOut, const double *rates, bool host, bool wait, const int *list = nullptr, int n = 0,
+                    const short *in16 = nullptr, short *out16 = nullptr) {
 	const Cfg &g = e->cfg;
 	const long long C = g.C;
 	const int inLat = g.B - g.B / 2, outLat = g.B / 2 + (g.split ? g.H : 0);
@@ -1400,6 +1420,7 @@ static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStri
 		}
 		if ((rc = stage_in(e, nullptr, inStride))) return rc; // capacity only
 		if ((rc = stage_out(e, outStride))) return rc;
+		if ((in16 || out16) && (rc = stage_pcm16(e, (size_t)P * C * std::max(inStride, 1), (size_t)P * C * std::max(outStride, 1)))) return rc;
 	}
 	// (sized by b200s_reserve: no allocation then)
 	if ((opsUsed & B200S_OPBIT(B200S_OP_FLUSH)) && (rc = ensure_buf(e, &e->dZero, &e->zeroCap, (size_t)std::max(zeroLen, 1), true))) return rc;
@@ -1462,13 +1483,19 @@ static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStri
 		d[s] = c;
 	}
 	if (host && !phases && anyPass) { // the stream groups copy their own slabs in and out
-		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, in, out, nullptr, nullptr, d, 1, lk, outStride, list, n))) return rc;
+		if ((rc = process_impl(e, dIn, inStride, C * inStride, inStride, dOut, outStride, C * outStride, outStride, in, out, in16, out16, d, 1, lk, outStride, list, n))) return rc;
 		if (wait) CK(cudaStreamSynchronize(e->stream));
 		return 0;
 	}
 	if (host) {
 		e->chainedGroups = 0;
 		if (in && inStride > 0) CK(cudaMemcpyAsync(e->dIn, in, sizeof(float) * (size_t)P * C * inStride, cudaMemcpyHostToDevice, e->stream));
+		if (in16 && inStride > 0) { // (before the pre phase: k_seek reads the seeks' rows)
+			const size_t cnt = (size_t)P * C * inStride;
+			CK(cudaMemcpyAsync(e->dIn16, in16, sizeof(short) * cnt, cudaMemcpyHostToDevice, e->stream));
+			B200S_LAUNCH(k_pcm16_in, dim3((unsigned)std::min<size_t>((cnt + 1023) / 1024, 4096)), dim3(256), 0, e->stream, (const short *)e->dIn16, e->dIn, cnt);
+			CKL();
+		}
 	}
 	if (phases) { // the whole table on the main stream, ahead of the pre phase (the call joins)
 		e->chainedGroups = 0;
@@ -1517,6 +1544,12 @@ static int run_impl(b200s_engine *e, const int *ops, const float *in, int inStri
 	if (pOut != dOut && outStride > 0)
 		PROF(PK_PHASE, B200S_LAUNCH(k_copy_rows, dim3((unsigned)std::min<long long>((long long)P * C, 65535)), dim3(256), 0, e->stream, dOut, outStride, (const float *)pOut, W, outStride, (int)(P * C)));
 	if (host && out && outStride > 0) CK(cudaMemcpyAsync(out, e->dOut, sizeof(float) * (size_t)P * C * outStride, cudaMemcpyDeviceToHost, e->stream));
+	if (host && out16 && outStride > 0) { // (after the post phase and k_copy_rows: the rows are final only now)
+		const size_t cnt = (size_t)P * C * outStride;
+		B200S_LAUNCH(k_pcm16_out, dim3((unsigned)std::min<size_t>((cnt + 1023) / 1024, 4096)), dim3(256), 0, e->stream, (const float *)e->dOut, e->dOut16, cnt);
+		CKL();
+		CK(cudaMemcpyAsync(out16, e->dOut16, sizeof(short) * cnt, cudaMemcpyDeviceToHost, e->stream));
+	}
 	if (wait) CK(cudaStreamSynchronize(e->stream));
 	return 0;
 }
@@ -2129,14 +2162,7 @@ int b200s_process_pcm16(b200s_engine *e, const short *in, int nIn, short *out, i
 	if (ci > e->inCap || co > e->outCap || ci > e->in16Cap || co > e->out16Cap || !e->dIn || !e->dOut) CK(cudaStreamSynchronize(e->stream)); // staging grows: drain first
 	if ((rc = stage_in(e, nullptr, nIn))) return rc;
 	if ((rc = stage_out(e, nOut))) return rc;
-	if (ci > e->in16Cap) {
-		if ((rc = dalloc(e, &e->dIn16, ci))) return rc;
-		e->in16Cap = ci;
-	}
-	if (co > e->out16Cap) {
-		if ((rc = dalloc(e, &e->dOut16, co))) return rc;
-		e->out16Cap = co;
-	}
+	if ((rc = stage_pcm16(e, ci, co))) return rc;
 	if ((rc = process_impl(e, e->dIn, nIn, (long long)e->cfg.C * nIn, nIn, e->dOut, nOut, (long long)e->cfg.C * nOut, nOut, nullptr, nullptr, in, out))) return rc;
 	if (wait) CK(cudaStreamSynchronize(e->stream));
 	return 0;
@@ -2186,11 +2212,12 @@ static int check_run(b200s_engine *e, const char *fn, const int *ops, int inStri
 	return 0;
 }
 static int run_entry(b200s_engine *e, const char *fn, const int *ops, const float *in, int inStride, const int *nIn, float *out,
-                     int outStride, const int *nOut, const double *rates, bool host, bool wait) {
+                     int outStride, const int *nOut, const double *rates, bool host, bool wait, const short *in16 = nullptr,
+                     short *out16 = nullptr) {
 	NEED_CFG();
 	int rc;
 	if ((rc = check_run(e, fn, ops, inStride, nIn, outStride, nOut, rates))) return rc;
-	return run_impl(e, ops, in, inStride, nIn, out, outStride, nOut, rates, host, wait);
+	return run_impl(e, ops, in, inStride, nIn, out, outStride, nOut, rates, host, wait, nullptr, 0, in16, out16);
 }
 int b200s_run_per_stream(b200s_engine *e, const int *ops, const float *in, int inStride, const int *nIn, float *out, int outStride,
                          const int *nOut, const double *rates) {
@@ -2206,7 +2233,8 @@ int b200s_run_per_stream_device(b200s_engine *e, const int *ops, const float *dI
 }
 // b200s_run_per_stream over a list of streams
 static int run_streams_entry(b200s_engine *e, const char *fn, int n, const int *streams, const int *ops, const float *in, int inStride,
-                             const int *nIn, float *out, int outStride, const int *nOut, const double *rates, bool host, bool wait) {
+                             const int *nIn, float *out, int outStride, const int *nOut, const double *rates, bool host, bool wait,
+                             const short *in16 = nullptr, short *out16 = nullptr) {
 	NEED_CFG();
 	if (n < 0 || n > e->S) {
 		e->err = std::string(fn) + ": n = " + std::to_string(n) + " is outside [0, " + std::to_string(e->S) + "]";
@@ -2216,7 +2244,7 @@ static int run_streams_entry(b200s_engine *e, const char *fn, int n, const int *
 	int rc;
 	if ((rc = check_run(e, fn, ops, inStride, nIn, outStride, nOut, rates, streams, n))) return rc;
 	if (n == 0) return 0;
-	return run_impl(e, ops, in, inStride, nIn, out, outStride, nOut, rates, host, wait, streams, n);
+	return run_impl(e, ops, in, inStride, nIn, out, outStride, nOut, rates, host, wait, streams, n, in16, out16);
 }
 int b200s_run_streams(b200s_engine *e, int n, const int *streams, const int *ops, const float *in, int inStride, const int *nIn,
                       float *out, int outStride, const int *nOut, const double *rates) {
@@ -2229,6 +2257,16 @@ int b200s_run_streams_async(b200s_engine *e, int n, const int *streams, const in
 int b200s_run_streams_device(b200s_engine *e, int n, const int *streams, const int *ops, const float *dIn, int inStride, const int *nIn,
                              float *dOut, int outStride, const int *nOut, const double *rates) {
 	return run_streams_entry(e, "b200s_run_streams_device", n, streams, ops, dIn, inStride, nIn, dOut, outStride, nOut, rates, false, false);
+}
+// 16-bit PCM host buffers (the conversions of b200s_process_pcm16, on the device)
+int b200s_run_per_stream_pcm16(b200s_engine *e, const int *ops, const short *in, int inStride, const int *nIn, short *out, int outStride,
+                               const int *nOut, const double *rates, int wait) {
+	return run_entry(e, "b200s_run_per_stream_pcm16", ops, nullptr, inStride, nIn, nullptr, outStride, nOut, rates, true, wait != 0, in, out);
+}
+int b200s_run_streams_pcm16(b200s_engine *e, int n, const int *streams, const int *ops, const short *in, int inStride, const int *nIn,
+                            short *out, int outStride, const int *nOut, const double *rates, int wait) {
+	return run_streams_entry(e, "b200s_run_streams_pcm16", n, streams, ops, nullptr, inStride, nIn, nullptr, outStride, nOut, rates, true,
+	                         wait != 0, in, out);
 }
 // process() with per-stream lengths: b200s_run_per_stream with every op PROCESS
 int b200s_process_per_stream(b200s_engine *e, const float *in, int inStride, const int *nIn, float *out, int outStride, const int *nOut) {
